@@ -1,4 +1,4 @@
-"""In-tree build of libb200vc.so (sm_100a only).
+"""In-tree build of libb200vc.so (sm_90a only).
 
 `python -m aicovergen_b200.build` or `__graft_entry__.build()`.  nvcc
 cross-compiles without a GPU; the resulting .so is git-ignored but travels with
@@ -19,7 +19,7 @@ OUT_DIR = PKG / "lib"
 LIB = OUT_DIR / "libb200vc.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -71,7 +71,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
 
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(compile_one, srcs))
-    cmd = [nvcc, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,11 +1,11 @@
-"""B200-native crepe F0 estimator for `f0_method="mangio-crepe"` — stands where `torchcrepe.predict(...)` stands in
+"""GPU-native crepe F0 estimator for `f0_method="mangio-crepe"` — stands where `torchcrepe.predict(...)` stands in
 `VC.get_f0_crepe_computation` (vc_infer_pipeline.py:96-137; `torchcrepe==0.0.20`, requirements.txt:19, model 'full').
 
-torchcrepe is a third-party dependency that is not under /root/reference; its published algorithm is restated (see
+torchcrepe is a third-party dependency that is not in the reference repository; its published algorithm is restated (see
 oracle/crepe.py for the line-by-line CPU restatement and the PARITY UNPINNED note):
 
   frames of 1024 samples @16 kHz every `hop_length`, zero-padded by 512, each mean/std normalised        b200vc_crepe_frames
-  6 x [pad, Conv2d(k x 1), ReLU, BatchNorm, MaxPool(2,1)]  (1024,128,128,128,256,512 ch; k = 512 s4, then 64)   tap-GEMMs on tcgen05
+  6 x [pad, Conv2d(k x 1), ReLU, BatchNorm, MaxPool(2,1)]  (1024,128,128,128,256,512 ch; k = 512 s4, then 64)   tap-GEMMs on the tensor cores
                                                                                      + b200vc_maxpool2_affine (BN after ReLU + pool)
   Linear(2048, 360) + sigmoid                                                          tap-GEMM epilogue
   bins outside [fmin, fmax) -> -inf, softmax, log                                      b200vc_crepe_logprob

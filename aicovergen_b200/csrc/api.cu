@@ -36,7 +36,7 @@ using namespace b200vc;
 
 extern "C" {
 
-const char* b200vc_version(void) { return "b200vc 0.1 (sm_100a)"; }
+const char* b200vc_version(void) { return "b200vc 0.1 (sm_90a)"; }
 const char* b200vc_last_error(void) { return g_err; }
 int64_t b200vc_launch_count(void) { return (int64_t)g_launches.load(); }
 void b200vc_count_launches(int64_t n) { g_launches.fetch_add((long long)n, std::memory_order_relaxed); }

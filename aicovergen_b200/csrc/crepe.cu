@@ -1,5 +1,5 @@
 // Row kernels of the crepe F0 path (`f0_method="mangio-crepe"`, vc_infer_pipeline.py:96-137 -> torchcrepe.predict).
-// The six convolutions and the classifier of torchcrepe's Crepe('full') run as tap-GEMMs on tcgen05; what is left is
+// The six convolutions and the classifier of torchcrepe's Crepe('full') run as tap-GEMMs on the tensor cores; what is left is
 // framing + per-frame normalisation, the (ReLU ->) BatchNorm -> MaxPool tail of every layer, the masked softmax / log of
 // the decoder input and the Viterbi recursion itself (librosa.sequence.viterbi with torchcrepe's banded transition).
 #include "common.cuh"

@@ -199,9 +199,8 @@ bigru_kernel(const float* __restrict__ xp, const float* __restrict__ whh /*[2][3
 //     data and its arrival signal travel together; each CTA waits on its OWN mbarrier for the 1024 bytes of the new h
 //     (armed one step ahead) instead of a cluster-wide barrier.  Double-buffered h: a CTA can only start step s+1 after
 //     every peer has SENT its step-s slice, which each peer does after its last read of the step-s input buffer.
-// Measured r02d on B200: 24 608 steps (4-min song) take 82 ms = 3.3 us/step — SLOWER than v1 (1.3 us/step): one st.async per
-// (unit, peer) means 256 remote mbarrier updates per CTA and step.  Not the default; a bulk-copy variant (one 128-byte
-// cp.async.bulk per peer) is the next thing to try.
+// One st.async per (unit, peer) means 256 remote mbarrier updates per CTA and step, which can cost more than v1's one
+// cluster barrier per step.  Not the default; v3 sends one 128-byte cp.async.bulk per peer instead.
 // ---------------------------------------------------------------------------
 constexpr int GRU2_THREADS = 512;
 
@@ -568,8 +567,7 @@ int b200vc_bigru(const float* xp, const float* whh, const float* bhh, float* out
   B200VC_RECORD(b200vc_bigru(xp, whh, bhh, out, T, hidden, stream));
   B200VC_REQUIRE(xp && whh && bhh && out && T > 0, "bigru: bad args");
   B200VC_REQUIRE(hidden == GRU_H, "bigru: hidden size %d unsupported (kernel is specialised for %d)", hidden, GRU_H);
-  // v2 (st.async + mbarrier per step) measured SLOWER on B200 (r02d: 3.3 us/step vs 1.3 us/step for v1: 256 remote
-  // complete_tx updates per CTA and step cost more than one cluster barrier); kept behind B200VC_GRU=2 (v3: B200VC_GRU=3) for experiments
+  // v2 (st.async + mbarrier per step) and v3 (bulk copy per peer) are kept behind B200VC_GRU=2 / 3 for experiments
   const char* e = getenv("B200VC_GRU");                 // 1 (default) | 2 | 3: exchange variant, see the kernels above
   const int ver = (e && (e[0] == '2' || e[0] == '3')) ? e[0] - '0' : 1;
   if (ver == 1) bigru_kernel<<<2 * GRU_CL, GRU_THREADS, 0, (cudaStream_t)stream>>>(xp, whh, bhh, out, T);

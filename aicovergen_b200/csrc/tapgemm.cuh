@@ -7,8 +7,8 @@
 //   out-of-range coordinates read as zero (this is the conv zero padding).
 // * Output pixels are tiled BW x BH (BW*BH == 128 GEMM rows per tile).
 // * The epilogue (bias / activation / residuals / scale / second output) is
-//   shared verbatim by the SIMT fp32 kernel and the tcgen05 TF32 kernel so both
-//   produce the same graph semantics.
+//   shared verbatim by the SIMT fp32 kernel and the wgmma tensor-core kernels so
+//   all produce the same graph semantics.
 //
 // Reference call sites this replaces (all cuDNN/cuBLAS library calls there):
 //   infer_pack/modules.py:299-312 (ResBlock1 convs), models.py:494-516
@@ -189,32 +189,14 @@ __device__ __forceinline__ void tg_act_vec(float (&v)[NV], int act, float prm) {
   }
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one lane moves a whole 32-byte sector, so a row-per-lane
-// epilogue issues full-sector requests instead of two 16-byte halves of every sector.
-__device__ __forceinline__ void tg_ldg256(float* d, const float* p) {
-  asm volatile("ld.global.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7])
-               : "l"(p));
-}
-__device__ __forceinline__ void tg_stg256(float* p, const float* v) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]),
-               "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
-               : "memory");
-}
-
 // 16 values <- 16 consecutive n at `ptr` with element stride `sn` (vector loads when the caller knows sn == 1 and the
-// address is 16-byte aligned; 256-bit when it is 32-byte aligned).
-__device__ __forceinline__ void tg_load16(float (&d)[16], const float* ptr, long long sn, bool vec, bool wide) {
+// address is 16-byte aligned).
+__device__ __forceinline__ void tg_load16(float (&d)[16], const float* ptr, long long sn, bool vec) {
   if (vec) {
-    if (wide && (reinterpret_cast<uintptr_t>(ptr) & 31) == 0) {
-      tg_ldg256(d, ptr);
-      tg_ldg256(d + 8, ptr + 8);
-    } else {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float4 t = reinterpret_cast<const float4*>(ptr)[j];
-        d[4 * j] = t.x; d[4 * j + 1] = t.y; d[4 * j + 2] = t.z; d[4 * j + 3] = t.w;
-      }
+    for (int j = 0; j < 4; ++j) {
+      const float4 t = reinterpret_cast<const float4*>(ptr)[j];
+      d[4 * j] = t.x; d[4 * j + 1] = t.y; d[4 * j + 2] = t.z; d[4 * j + 3] = t.w;
     }
   } else {
 #pragma unroll
@@ -240,19 +222,14 @@ __device__ __forceinline__ void tg_load16h(float (&d)[16], const __half* ptr, lo
     for (int j = 0; j < 16; ++j) d[j] = __half2float(ptr[j * sn]);
   }
 }
-__device__ __forceinline__ void tg_put16(float* ptr, long long sn, bool vec, bool rnd, bool wide, const float (&v)[16]) {
+__device__ __forceinline__ void tg_put16(float* ptr, long long sn, bool vec, bool rnd, const float (&v)[16]) {
   if (vec) {
     float w[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) w[j] = rnd ? round_tf32(v[j]) : v[j];
-    if (wide && (reinterpret_cast<uintptr_t>(ptr) & 31) == 0) {
-      tg_stg256(ptr, w);
-      tg_stg256(ptr + 8, w + 8);
-    } else {
-      float4* op = reinterpret_cast<float4*>(ptr);
+    float4* op = reinterpret_cast<float4*>(ptr);
 #pragma unroll
-      for (int j = 0; j < 4; ++j) op[j] = make_float4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
-    }
+    for (int j = 0; j < 4; ++j) op[j] = make_float4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
   } else {
     // transposed layouts: consecutive lanes own consecutive pixels, so each of these scalar stores is lane-coalesced
     if (rnd) {
@@ -272,31 +249,19 @@ __device__ __forceinline__ void tg_put16h(__half* ptr, long long sn, bool vec, c
       const __half2 h = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
       w[i] = *reinterpret_cast<const uint32_t*>(&h);
     }
-    if ((reinterpret_cast<uintptr_t>(ptr) & 31) == 0) {
-      // 16 halfs = one 32-byte sector: a single 256-bit store writes it whole (ncu r02a: two 16-byte stores per lane made
-      // every L2 write a half-sector, 32 sectors per request at 50 % utilisation)
-      asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(ptr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-                   "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-                   : "memory");
-    } else {
-      reinterpret_cast<uint4*>(ptr)[0] = make_uint4(w[0], w[1], w[2], w[3]);
-      reinterpret_cast<uint4*>(ptr)[1] = make_uint4(w[4], w[5], w[6], w[7]);
-    }
+    reinterpret_cast<uint4*>(ptr)[0] = make_uint4(w[0], w[1], w[2], w[3]);
+    reinterpret_cast<uint4*>(ptr)[1] = make_uint4(w[4], w[5], w[6], w[7]);
   } else {
 #pragma unroll
     for (int j = 0; j < 16; ++j) ptr[j * sn] = __float2half_rn(v[j]);
   }
 }
 
-// Store 16 consecutive n (n % 16 == 0) of one GEMM row straight from accumulator registers: the epilogue the tcgen05
-// kernels use (one thread owns one TMEM lane = one row).  Every stage is a pass over the register array behind a
-// warp-uniform test, so a plain bias+activation epilogue is ~5 instructions per element.  Same arithmetic, in the same
-// order, as tg_epi1.
-// `pre_bias`: the 16 per-column biases already in registers (persistent kernels whose warps keep the same columns).
-// `wide`: 256-bit accesses where the row pointer is 32-byte aligned.  Measured (r01, bench_tapgemm): +4..18 % on the
-// persistent kernel, -18 % on the weight-stationary kernel with 128-byte rows (N = 32), neutral for N = 64.
-__device__ __forceinline__ void tg_store16(const TgParams& p, const TgRow& r, int n, const uint32_t* acc,
-                                           const float* pre_bias = nullptr, bool wide = false) {
+// Store 16 consecutive n (n % 16 == 0) of one GEMM row from registers: the epilogue the wgmma kernels use after
+// regrouping their accumulator fragments so that one thread owns one row (hopper.cuh, wg_epilogue).  Every stage is a
+// pass over the register array behind a warp-uniform test, so a plain bias+activation epilogue is ~5 instructions per
+// element.  Same arithmetic, in the same order, as tg_epi1.
+__device__ __forceinline__ void tg_store16(const TgParams& p, const TgRow& r, int n, const uint32_t* acc) {
   if (!r.valid || n >= p.N) return;
   if (n + 15 >= p.N) {      // ragged tail of N: element-wise path with bounds checks
 #pragma unroll
@@ -311,7 +276,7 @@ __device__ __forceinline__ void tg_store16(const TgParams& p, const TgRow& r, in
   for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(acc[j]);
   if (p.acc_in) {            // partial sums of earlier launches (split reduction), added in fp32 round-to-nearest
     float pa[16];
-    tg_load16(pa, p.acc_in + r.a_off + n, 1, true, wide);
+    tg_load16(pa, p.acc_in + r.a_off + n, 1, true);
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] += pa[j];
   }
@@ -320,10 +285,7 @@ __device__ __forceinline__ void tg_store16(const TgParams& p, const TgRow& r, in
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] *= rs;
   }
-  if (pre_bias) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] += pre_bias[j];
-  } else if (p.bias) {
+  if (p.bias) {
     if (p.bias_per_row) {
       const float bb = __ldg(p.bias + r.brow);
 #pragma unroll
@@ -348,10 +310,10 @@ __device__ __forceinline__ void tg_store16(const TgParams& p, const TgRow& r, in
   if (p.res) {
     float rr[16];
     if (p.dtype & TG_DT_RES) tg_load16h(rr, reinterpret_cast<const __half*>(p.res) + r.r_off + n * p.r_sn, p.r_sn, (p.vec4 & TG_VEC_RES) != 0);
-    else tg_load16(rr, p.res + r.r_off + n * p.r_sn, p.r_sn, (p.vec4 & TG_VEC_RES) != 0, wide);
+    else tg_load16(rr, p.res + r.r_off + n * p.r_sn, p.r_sn, (p.vec4 & TG_VEC_RES) != 0);
     if (p.split & 2) {        // split residual: hi + lo
       float r2[16];
-      tg_load16(r2, p.res + r.r_off + n * p.r_sn + p.r_split, p.r_sn, (p.vec4 & TG_VEC_RES) != 0, wide);
+      tg_load16(r2, p.res + r.r_off + n * p.r_sn + p.r_split, p.r_sn, (p.vec4 & TG_VEC_RES) != 0);
 #pragma unroll
       for (int j = 0; j < 16; ++j) rr[j] += r2[j];
     }
@@ -371,7 +333,7 @@ __device__ __forceinline__ void tg_store16(const TgParams& p, const TgRow& r, in
   if (p.res2) {
     float rr[16];
     if (p.dtype & TG_DT_RES2) tg_load16h(rr, reinterpret_cast<const __half*>(p.res2) + r.o_off + n * p.o_sn, p.o_sn, vec);
-    else tg_load16(rr, p.res2 + r.o_off + n * p.o_sn, p.o_sn, vec, wide);
+    else tg_load16(rr, p.res2 + r.o_off + n * p.o_sn, p.o_sn, vec);
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] += rr[j];
   }
@@ -381,26 +343,26 @@ __device__ __forceinline__ void tg_store16(const TgParams& p, const TgRow& r, in
 #pragma unroll
     for (int j = 0; j < 16; ++j) { hi[j] = round_tf32(v[j]); lo[j] = round_tf32(v[j] - hi[j]); }
     float* o = p.out + r.o_off + n * p.o_sn;
-    tg_put16(o, p.o_sn, vec, false, wide, hi);
-    tg_put16(o + p.o_split, p.o_sn, vec, false, wide, lo);
-    tg_put16(o + 2 * p.o_split, p.o_sn, vec, false, wide, hi);
+    tg_put16(o, p.o_sn, vec, false, hi);
+    tg_put16(o + p.o_split, p.o_sn, vec, false, lo);
+    tg_put16(o + 2 * p.o_split, p.o_sn, vec, false, hi);
     return;
   }
   if (p.dtype & TG_DT_OUT) tg_put16h(reinterpret_cast<__half*>(p.out) + r.o_off + n * p.o_sn, p.o_sn, vec, v);
-  else tg_put16(p.out + r.o_off + n * p.o_sn, p.o_sn, vec, (p.round_tf32 & 1) != 0, wide, v);
+  else tg_put16(p.out + r.o_off + n * p.o_sn, p.o_sn, vec, (p.round_tf32 & 1) != 0, v);
   if (p.out2) {
     tg_act_vec(v, p.act2, p.act2_p);
     const long long sn2 = p.out2_own ? p.o2_sn : p.o_sn;
     const bool vec2 = p.out2_own ? (p.vec4 & TG_VEC_OUT2) != 0 : vec;
     if (p.dtype & TG_DT_OUT2) tg_put16h(reinterpret_cast<__half*>(p.out2) + r.o2_off + n * sn2, sn2, vec2, v);
-    else tg_put16(p.out2 + r.o2_off + n * sn2, sn2, vec2, (p.round_tf32 & 2) != 0, wide, v);
+    else tg_put16(p.out2 + r.o2_off + n * sn2, sn2, vec2, (p.round_tf32 & 2) != 0, v);
   }
 }
 
-// Host-side launchers (tapgemm_simt.cu / tapgemm_tc.cu).
+// Host-side launchers (tapgemm_simt.cu / tapgemm_tc.cu / tapgemm_ws.cu).
 int tapgemm_simt_launch(const TgParams& p, cudaStream_t stream);
 int tapgemm_tc_launch(const TgParams& p, cudaStream_t stream);    // v1: one tile per CTA
-int tapgemm_tc2_launch(const TgParams& p, cudaStream_t stream);   // v2: persistent, double-buffered TMEM, coalesced epilogue
+int tapgemm_tc2_launch(const TgParams& p, cudaStream_t stream);   // v2: persistent (one CTA per SM walks the tiles)
 bool tapgemm_tc_supported(const TgParams& p);
 void tapgemm_tc2_set_rows256(int on);                            // experimental 256-row tiles of the persistent kernel
 int tapgemm_ws_launch(const TgParams& p, cudaStream_t stream);    // v3: weight-stationary + halo (small-channel convs)

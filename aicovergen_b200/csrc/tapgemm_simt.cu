@@ -1,5 +1,5 @@
 // fp32 SIMT tap-GEMM: exact-fp32 path (rmvpe, IVF coarse quantiser, small-K
-// layers) and the on-device cross-check for the tcgen05 kernel.
+// layers) and the on-device cross-check for the wgmma kernels.
 // 128 x BN output tile, BK = 16, 256 threads, 8 x (BN/16) register tile,
 // register-prefetch double buffering.
 #include "tapgemm.cuh"

@@ -1,271 +1,163 @@
-// tcgen05 / TMEM / TMA tap-GEMM for sm_100a (TF32 inputs, fp32 accumulate).
+// wgmma / TMA tap-GEMM for sm_90a (TF32 or fp16 operands, fp32 accumulate).
 //
-// One CTA = one 128 x BN output tile.  Warp-specialised:
-//   warp 0      : TMA producer  (cp.async.bulk.tensor 5-D box of A per tap/k-chunk,
-//                 3-D box of W), mbarrier complete_tx
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (kind::tf32,
-//                 cta_group::1, M=128, N=BN, K=8 per instruction, 4 per 128-byte
-//                 swizzle atom), tcgen05.commit releases smem stages
-//   warps 2..5  : epilogue - tcgen05.ld 32x32b.x32 from TMEM, fused epilogue
-//                 (tapgemm.cuh), vectorised global stores
+// One CTA = three warpgroups:
+//   warpgroup 0    : TMA producer (one thread): per tap and 128-byte K chunk a 5-D box of A (the tile's pixels) and a
+//                    3-D box of W into a ring of shared-memory stages, mbarrier complete_tx
+//   warpgroups 1-2 : consumers: each issues m64 x BN wgmma for its 64 rows of every 128-row block of the tile straight from
+//                    the ring (descriptors, no register staging of operands), releases a stage once the wgmma that read it
+//                    has retired, then runs the fused epilogue (tapgemm.cuh) on its accumulator registers
 //
-// A pixels x 32 channels land in shared memory as 128 rows x 128 B with the
-// hardware 128-byte swizzle, which is exactly the canonical K-major SWIZZLE_128B
-// UMMA operand layout: conv zero padding comes for free from TMA's
-// out-of-bounds zero fill, so no im2col buffer ever exists in HBM.
-#include "tapgemm.cuh"
-#include <cuda.h>
+// A pixels x 32 fp32 (64 fp16) channels land in shared memory as rows of 128 B with the hardware 128-byte swizzle, which is
+// the canonical K-major SWIZZLE_128B wgmma operand layout: conv zero padding comes for free from TMA's out-of-bounds zero
+// fill, so no im2col buffer ever exists in HBM.
+//
+// The same kernel serves both launch forms: one tile per CTA (tapgemm_tc_launch) and persistent, one CTA per SM walking
+// the tiles with the n-tile fastest so neighbouring CTAs share the A box in L2 (tapgemm_tc2_launch).
+#include "hopper.cuh"
+#include <cstdlib>
 
 namespace b200vc {
 
+using namespace hop;
+
 namespace {
 
-constexpr int KCHUNK = 32;                  // fp32 elements per 128-byte swizzle row
-constexpr int A_STAGE_BYTES = TG_TILE_M * 128;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 3 * WG_THREADS;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "LAB_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE;\n\t"
-      "bra LAB_WAIT;\n\t"
-      "DONE:\n\t"
-      "}" ::"r"(bar), "r"(parity)
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm, uint32_t bar,
-                                            int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm, uint32_t bar,
-                                            int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 "version 1").
-//   start address >> 4 in [0,14); LBO(unused for swizzled K-major)=1 in [16,30);
-//   SBO = 1024 B (8 rows x 128 B) >> 4 in [32,46); version=1 in [46,48);
-//   layout type SWIZZLE_128B = 2 in [61,64).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Instruction descriptor: D=F32 (bits 4-5 = 1), A=B=TF32 (format 2 at bits 7-9, 10-12),
-// both K-major, N>>3 at bits 17-22, M>>4 at bits 24-28.
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(NUM_THREADS)
-tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
-                  const __grid_constant__ TgParams p) {
+// MH = 128-row blocks per tile: with MH == 2 one W tile feeds the MMAs of 256 rows.
+template <int BN, int STAGES, int MH, bool F16>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+tapgemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
+                  const __grid_constant__ TgParams p, int ntiles_n, int total_tiles, int tbw, int tbh) {
+  constexpr int KE = F16 ? 2 * KCHUNK : KCHUNK;                    // K elements per 128-byte chunk row
+  constexpr int ES = F16 ? 2 : 4;
+  constexpr int A_STAGE_BYTES = MH * TG_TILE_M * 128;
   constexpr int B_STAGE_BYTES = BN * 128;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
-  constexpr uint32_t IDESC = make_idesc_tf32(128, BN);
-
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment required by the 128-byte swizzle atoms.
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
+  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
+  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES + 2 * STG_BYTES;
   auto a_stage = [&](int s) { return smem_base + s * STAGE_BYTES; };
   auto b_stage = [&](int s) { return smem_base + s * STAGE_BYTES + A_STAGE_BYTES; };
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t tmem_full_bar = bar_base + 8u * (2 * STAGES);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 1);
 
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
-
-  // ---- tile coordinates
-  const int ntw = (p.OW + p.BW - 1) / p.BW;
-  const int nth = (p.OH + p.BH - 1) / p.BH;
-  int tile = blockIdx.x;
-  const int tw = tile % ntw; tile /= ntw;
-  const int th = tile % nth; tile /= nth;
-  const int tb = tile;
-  const int w0 = tw * p.BW, h0 = th * p.BH;
-  const int n0 = blockIdx.y * BN;
-
-  const int kchunks = (p.Kc + KCHUNK - 1) / KCHUNK;
+  const int wg = threadIdx.x / WG_THREADS;
+  const int ntw = (p.OW + tbw - 1) / tbw;
+  const int nth = (p.OH + tbh - 1) / tbh;
+  const int kchunks = (p.Kc + KE - 1) / KE;
   const int nchunks = p.ntaps * kchunks;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
+  if (threadIdx.x == 0) {
+    prefetch_tensormap(&tmA);
+    prefetch_tensormap(&tmW);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);              // one arrival per consumer warp
     }
-    mbar_init(tmem_full_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                 "r"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
+  auto tile_coords = [&](int tile, int& w0, int& h0, int& tb, int& n0) {
+    const int nt = tile % ntiles_n;
+    int mt = tile / ntiles_n;
+    const int tw = mt % ntw; mt /= ntw;
+    const int th = mt % nth; mt /= nth;
+    tb = mt;
+    w0 = tw * tbw;
+    h0 = th * tbh;
+    n0 = nt * BN;
+  };
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    {
-      int s = 0;
-      uint32_t ph = 0;
+    setmaxnreg_dec<40>();                      // registers go to the consumers' accumulators
+    if (threadIdx.x != 0) return;
+    int s = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      int w0, h0, tb, n0;
+      tile_coords(tile, w0, h0, tb, n0);
       const int wsel = tb * p.w_batch_step;
       for (int tap_i = 0; tap_i < p.ntaps; ++tap_i) {
         const TgTap tap = p.taps[tap_i];
         const int cw = w0 + tap.dw, ch = h0 + tap.dh, cp = tap.dp, widx = tap.widx + wsel;
         int ca = tap.c_off;
-        for (int kc0 = 0; kc0 < p.Kc; kc0 += KCHUNK, ca += KCHUNK) {
+        for (int kc0 = 0; kc0 < p.Kc; kc0 += KE, ca += KE) {
           mbar_wait(empty_bar(s), ph ^ 1u);
-          if (elect_one()) {
-            mbar_expect_tx(full_bar(s), STAGE_BYTES);
-            tma_load_5d(a_stage(s), &tmA, full_bar(s), ca, cw, ch, tb, cp);
-            tma_load_3d(b_stage(s), &tmW, full_bar(s), kc0, n0, widx);
-          }
-          __syncwarp();
+          mbar_expect_tx(full_bar(s), STAGE_BYTES);
+          tma_load_5d(a_stage(s), &tmA, full_bar(s), ca, cw, ch, tb, cp);
+          tma_load_3d(b_stage(s), &tmW, full_bar(s), kc0, n0, widx);
           if (++s == STAGES) { s = 0; ph ^= 1u; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // whole warp walks the loop (uniform control flow -> descriptors stay in uniform registers); one elected lane issues
-    {
-      const int klast = ((p.Kc - (kchunks - 1) * KCHUNK) + 7) >> 3;   // short last k-chunk: only the K=8 steps with data
-      uint32_t accum = 0u;
-      int s = 0, kc = 0;
-      uint32_t ph = 0;
-      for (int chunk = 0; chunk < nchunks; ++chunk) {
-        mbar_wait(full_bar(s), ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int nk = (kc == kchunks - 1) ? klast : KCHUNK / 8;
-        if (elect_one()) {
-          const uint64_t adesc = make_smem_desc(a_stage(s));
-          const uint64_t bdesc = make_smem_desc(b_stage(s));
-          // advance 8 tf32 = 32 bytes inside the swizzle atom: +2 in the (addr >> 4) field
-          if (nk == KCHUNK / 8) {
-#pragma unroll
-            for (int k = 0; k < KCHUNK / 8; ++k) {
-              umma_tf32(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), IDESC, accum);
-              accum = 1u;
-            }
-          } else {
-            for (int k = 0; k < nk; ++k) {
-              umma_tf32(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), IDESC, accum);
-              accum = 1u;
-            }
-          }
-          umma_commit(empty_bar(s));   // frees this smem stage once the MMAs have read it
-          if (chunk == nchunks - 1) umma_commit(tmem_full_bar);    // accumulator complete
-        }
-        accum = 1u;
-        __syncwarp();
-        if (++s == STAGES) { s = 0; ph ^= 1u; }
-        if (++kc == kchunks) kc = 0;
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int m = q * 32 + lane;            // GEMM row inside the tile
-    const int h = h0 + m / p.BW, w = w0 + m % p.BW;
-    const TgRow r = tg_row(p, tb, h, w);
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      if (n0 + c0 >= p.N) break;            // warp-uniform
-      uint32_t v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-      tg_store16(p, r, n0 + c0, v);
-      tg_store16(p, r, n0 + c0 + 16, v + 16);
-    }
+    return;
   }
 
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(TMEM_COLS)
-                 : "memory");
+  // ===================== consumers (warpgroups 1, 2) =====================
+  setmaxnreg_inc<232>();
+  const int g = wg - 1;
+  const int t = threadIdx.x & (WG_THREADS - 1);
+  float* stg = reinterpret_cast<float*>(smem_gen + STAGES * STAGE_BYTES + g * STG_BYTES);
+  // the last k-chunk of a tap may be short (Kc = 48 -> 32 + 16): issue only the 32-byte K steps that hold data
+  const int klast = ((p.Kc - (kchunks - 1) * KE) * ES + 31) >> 5;
+  float acc[MH][BN / 2];
+#pragma unroll
+  for (int mh = 0; mh < MH; ++mh)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[mh][i] = 0.f;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    int w0, h0, tb, n0;
+    tile_coords(tile, w0, h0, tb, n0);
+    int prev = -1;
+    for (int chunk = 0, kc = 0; chunk < nchunks; ++chunk) {
+      mbar_wait(full_bar(s), ph);
+      const int nk = (kc == kchunks - 1) ? klast : 4;
+      const uint64_t adesc = make_desc(a_stage(s) + g * WG_ROWS * 128);
+      const uint64_t bdesc = make_desc(b_stage(s));
+#pragma unroll
+      for (int mh = 0; mh < MH; ++mh) fence_operands(acc[mh]);
+      wgmma_fence();
+      if (nk == 4) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+          for (int mh = 0; mh < MH; ++mh)      // 128 rows x 128 B = 16 KB further into the A box: +1024 in the (addr >> 4) field
+            wgmma<F16, BN>(acc[mh], adesc + (uint64_t)(mh * 1024 + 2 * k), bdesc + (uint64_t)(2 * k), (chunk | k) != 0);
+      } else {
+        for (int k = 0; k < nk; ++k)
+#pragma unroll
+          for (int mh = 0; mh < MH; ++mh)
+            wgmma<F16, BN>(acc[mh], adesc + (uint64_t)(mh * 1024 + 2 * k), bdesc + (uint64_t)(2 * k), (chunk | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                          // the previous chunk's wgmma have retired: its stage can be refilled
+#pragma unroll
+      for (int mh = 0; mh < MH; ++mh) fence_operands(acc[mh]);
+      if (prev >= 0) {
+        __syncwarp();
+        if ((t & 31) == 0) mbar_arrive(empty_bar(prev));
+      }
+      prev = s;
+      if (++s == STAGES) { s = 0; ph ^= 1u; }
+      if (++kc == kchunks) kc = 0;
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int mh = 0; mh < MH; ++mh) fence_operands(acc[mh]);
+    __syncwarp();
+    if ((t & 31) == 0) mbar_arrive(empty_bar(prev));
+#pragma unroll
+    for (int mh = 0; mh < MH; ++mh) {
+      const int m = mh * TG_TILE_M + g * WG_ROWS + (t & (WG_ROWS - 1));   // row inside the (tbw x tbh) box, w fastest
+      const TgRow r = tg_row(p, tb, h0 + m / tbw, w0 + m % tbw);
+      wg_epilogue<BN>(p, r, n0, acc[mh], stg, 1 + g);
+    }
   }
 }
 
@@ -318,21 +210,94 @@ int encode_map(CUtensorMap* tm, const void* base, int rank, const cuuint64_t* di
   return kOk;
 }
 
-template <int BN, int STAGES>
-int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmW, const TgParams& p, dim3 grid,
-               cudaStream_t stream) {
-  constexpr int smem = STAGES * (A_STAGE_BYTES + BN * 128) + 8 * (2 * STAGES + 2) + 1024;
+constexpr int SMEM_LIMIT = 227 * 1024;
+
+template <int BN, int STAGES, int MH, bool F16>
+int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmW, const TgParams& p, int ntiles_n, int total_tiles,
+               int grid, int tbw, int tbh, cudaStream_t stream) {
+  constexpr int smem = STAGES * (MH * TG_TILE_M * 128 + BN * 128) + 2 * STG_BYTES + 8 * 2 * STAGES + 1024;
+  static_assert(smem <= SMEM_LIMIT, "shared memory budget");
   static bool configured = false;
   if (!configured) {
-    B200VC_CHECK_CUDA(cudaFuncSetAttribute(tapgemm_tc_kernel<BN, STAGES>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    B200VC_CHECK_CUDA(cudaFuncSetAttribute(tapgemm_wg_kernel<BN, STAGES, MH, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
-  tapgemm_tc_kernel<BN, STAGES><<<grid, NUM_THREADS, smem, stream>>>(tmA, tmW, p);
+  tapgemm_wg_kernel<BN, STAGES, MH, F16><<<grid, NUM_THREADS, smem, stream>>>(tmA, tmW, p, ntiles_n, total_tiles, tbw, tbh);
+  return kOk;
+}
+
+template <int MH, bool F16>
+int launch_bn(int BN, const CUtensorMap& tmA, const CUtensorMap& tmW, const TgParams& p, int ntiles_n, int total, int grid,
+              int tbw, int tbh, cudaStream_t stream) {
+  // ring depth: as many stages as fit beside the two 9 KB epilogue staging blocks (~192 KB of operands)
+  if constexpr (MH == 1) {
+    switch (BN) {
+      case 256: return launch_cfg<256, 4, 1, F16>(tmA, tmW, p, ntiles_n, total, grid, tbw, tbh, stream);
+      case 128: return launch_cfg<128, 6, 1, F16>(tmA, tmW, p, ntiles_n, total, grid, tbw, tbh, stream);
+      case 64:  return launch_cfg<64, 8, 1, F16>(tmA, tmW, p, ntiles_n, total, grid, tbw, tbh, stream);
+      default:  return launch_cfg<32, 8, 1, F16>(tmA, tmW, p, ntiles_n, total, grid, tbw, tbh, stream);
+    }
+  } else {
+    switch (BN) {       // 256-row tiles: two m64 accumulators per consumer thread, so at most 128 columns
+      case 128: return launch_cfg<128, 4, 2, F16>(tmA, tmW, p, ntiles_n, total, grid, tbw, tbh, stream);
+      case 64:  return launch_cfg<64, 5, 2, F16>(tmA, tmW, p, ntiles_n, total, grid, tbw, tbh, stream);
+      default:  return launch_cfg<32, 5, 2, F16>(tmA, tmW, p, ntiles_n, total, grid, tbw, tbh, stream);
+    }
+  }
+}
+
+int g_rows256 = [] { const char* e = getenv("B200VC_TC2_ROWS256"); return (e && e[0] == '1') ? 1 : 0; }();
+
+int tc_launch(const TgParams& p, cudaStream_t stream, bool persistent) {
+  B200VC_REQUIRE(tapgemm_tc_supported(p), "tapgemm_tc: operand alignment not TMA-compatible");
+  const bool f16 = (p.dtype & TG_DT_AB) != 0;
+  const int BN = p.N > 128 ? 256 : (p.N > 64 ? 128 : (p.N > 32 ? 64 : 32));
+  const int ntiles_n = ceil_div(p.N, BN);
+  // 256-row tiles (one W tile feeds the MMAs of two 128-row blocks) halve the W traffic per FLOP; experimental, off by
+  // default (b200vc_tapgemm_set_rows256, initial value from env B200VC_TC2_ROWS256), persistent launches only
+  int tbw = p.BW, tbh = p.BH, MH = 1;
+  if (persistent && g_rows256 && !f16 && BN <= 128) {
+    const int bw2 = p.BH == 1 ? 2 * p.BW : p.BW, bh2 = p.BH == 1 ? 1 : 2 * p.BH;
+    if (bw2 <= 256 && bh2 <= 256) {
+      const long long t1 = (long long)ceil_div(p.OW, p.BW) * ceil_div(p.OH, p.BH) * p.OB;
+      const long long t2 = (long long)ceil_div(p.OW, bw2) * ceil_div(p.OH, bh2) * p.OB;
+      if (t2 * ntiles_n >= num_sms() && 2 * t2 * 100 <= t1 * 105) { tbw = bw2; tbh = bh2; MH = 2; }
+    }
+  }
+  const long long total = (long long)ceil_div(p.OW, tbw) * ceil_div(p.OH, tbh) * p.OB * ntiles_n;
+  B200VC_REQUIRE(total > 0 && total < (1ll << 31), "tapgemm_tc: bad tile count %lld", total);
+
+  const cuuint32_t ke = f16 ? 2 * KCHUNK : KCHUNK;
+  CUtensorMap tmA, tmW;
+  const cuuint32_t abox[5] = {ke, (cuuint32_t)tbw, (cuuint32_t)tbh, 1, 1};
+  int rc = encode_a_map(&tmA, p, abox);
+  if (rc) return rc;
+  int max_widx = 0;
+  for (int i = 0; i < p.ntaps; ++i) max_widx = p.taps[i].widx > max_widx ? p.taps[i].widx : max_widx;
+  rc = encode_w_map(&tmW, p, max_widx + 1 + (p.OB - 1) * p.w_batch_step, p.wstride, (int)ke, BN);
+  if (rc) return rc;
+  const int grid = (int)(persistent && total > num_sms() ? num_sms() : total);
+  if (MH == 2) rc = launch_bn<2, false>(BN, tmA, tmW, p, ntiles_n, (int)total, grid, tbw, tbh, stream);
+  else if (f16) rc = launch_bn<1, true>(BN, tmA, tmW, p, ntiles_n, (int)total, grid, tbw, tbh, stream);
+  else rc = launch_bn<1, false>(BN, tmA, tmW, p, ntiles_n, (int)total, grid, tbw, tbh, stream);
+  if (rc) return rc;
+  count_launch();
+  B200VC_LAUNCH_CHECK();
   return kOk;
 }
 
 }  // namespace
+
+int num_sms() {
+  static int n = 0;
+  if (!n) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (n <= 0) n = 132;
+  }
+  return n;
+}
 
 int encode_map_f32(CUtensorMap* tm, const void* base, int rank, const cuuint64_t* dims,
                    const cuuint64_t* strides_bytes, const cuuint32_t* box) {
@@ -343,7 +308,42 @@ int encode_map_f16(CUtensorMap* tm, const void* base, int rank, const cuuint64_t
   return encode_map(tm, base, rank, dims, strides_bytes, box, true);
 }
 
-// Whether a problem can go through the TMA/tcgen05 path (alignment rules of
+namespace hop {
+
+int encode_a_map(CUtensorMap* tm, const TgParams& p, const cuuint32_t (&box)[5]) {
+  const bool f16 = (p.dtype & TG_DT_AB) != 0;
+  const unsigned long long es = f16 ? 2ull : 4ull;
+  const int epb = f16 ? 8 : 4;                           // elements per 16 bytes (TMA stride granule)
+  cuuint64_t dims[5], strides[4];
+  long long span = 1;                                    // safe stride for size-1 dims
+  for (int i = 0; i < 5; ++i) {
+    dims[i] = (cuuint64_t)(p.a_dim[i] > 0 ? p.a_dim[i] : 1);
+    if (i > 0) {
+      long long st = p.a_stride[i];
+      if (p.a_dim[i] <= 1) st = ((span + epb - 1) / epb) * epb;
+      strides[i - 1] = (cuuint64_t)st * es;
+      span = st * (long long)dims[i];
+    } else {
+      span = (long long)dims[0];
+    }
+  }
+  return encode_map(tm, p.A, 5, dims, strides, box, f16);
+}
+
+int encode_w_map(CUtensorMap* tm, const TgParams& p, int nw, long long wstride, int box_k, int box_n) {
+  const bool f16 = (p.dtype & TG_DT_AB) != 0;
+  const unsigned long long es = f16 ? 2ull : 4ull;
+  const int epb = f16 ? 8 : 4;
+  cuuint64_t dims[3] = {(cuuint64_t)p.Kc, (cuuint64_t)p.N, (cuuint64_t)nw};
+  if (nw <= 1) wstride = ((p.ldw * p.N + epb - 1) / epb) * epb;
+  cuuint64_t strides[2] = {(cuuint64_t)p.ldw * es, (cuuint64_t)wstride * es};
+  cuuint32_t box[3] = {(cuuint32_t)box_k, (cuuint32_t)box_n, 1};
+  return encode_map(tm, p.Wt, 3, dims, strides, box, f16);
+}
+
+}  // namespace hop
+
+// Whether a problem can go through the TMA/wgmma path (alignment rules of
 // cuTensorMapEncodeTiled); otherwise callers use the SIMT kernel.
 bool tapgemm_tc_supported(const TgParams& p) {
   const int epb = (p.dtype & TG_DT_AB) ? 8 : 4;            // elements per 16 bytes
@@ -357,58 +357,12 @@ bool tapgemm_tc_supported(const TgParams& p) {
 }
 
 int tapgemm_tc_launch(const TgParams& p, cudaStream_t stream) {
-  B200VC_REQUIRE(tapgemm_tc_supported(p), "tapgemm_tc: operand alignment not TMA-compatible");
   B200VC_REQUIRE(!(p.dtype & TG_DT_AB), "tapgemm_tc: fp16 operands are handled by the persistent / weight-stationary kernels");
-  const int ntw = ceil_div(p.OW, p.BW), nth = ceil_div(p.OH, p.BH);
-  const long long tiles = (long long)ntw * nth * p.OB;
-  B200VC_REQUIRE(tiles > 0 && tiles < (1ll << 31), "tapgemm_tc: bad tile count %lld", tiles);
-
-  // ---- A map: rank 5 (c, w, h, b, p)
-  CUtensorMap tmA, tmW;
-  {
-    cuuint64_t dims[5], strides[4];
-    cuuint32_t box[5] = {KCHUNK, (cuuint32_t)p.BW, (cuuint32_t)p.BH, 1, 1};
-    long long span = 1;  // safe stride for size-1 dims
-    for (int i = 0; i < 5; ++i) {
-      dims[i] = (cuuint64_t)(p.a_dim[i] > 0 ? p.a_dim[i] : 1);
-      if (i > 0) {
-        long long st = p.a_stride[i];
-        if (p.a_dim[i] <= 1) st = ((span + 3) / 4) * 4;
-        strides[i - 1] = (cuuint64_t)st * 4ull;
-        span = st * (long long)dims[i];
-      } else {
-        span = (long long)dims[0];
-      }
-    }
-    int rc = encode_map(&tmA, p.A, 5, dims, strides, box);
-    if (rc) return rc;
-  }
-  // ---- W map: rank 3 (k, n, widx)
-  int max_widx = 0;
-  for (int i = 0; i < p.ntaps; ++i) max_widx = p.taps[i].widx > max_widx ? p.taps[i].widx : max_widx;
-  const int nw = max_widx + 1 + (p.OB - 1) * p.w_batch_step;
-  const int BN = p.N > 128 ? 256 : (p.N > 64 ? 128 : (p.N > 32 ? 64 : 32));
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)p.Kc, (cuuint64_t)p.N, (cuuint64_t)nw};
-    long long wst = p.wstride;
-    if (nw <= 1) wst = ((p.ldw * p.N + 3) / 4) * 4;
-    cuuint64_t strides[2] = {(cuuint64_t)p.ldw * 4ull, (cuuint64_t)wst * 4ull};
-    cuuint32_t box[3] = {KCHUNK, (cuuint32_t)BN, 1};
-    int rc = encode_map(&tmW, p.Wt, 3, dims, strides, box);
-    if (rc) return rc;
-  }
-  dim3 grid((unsigned)tiles, ceil_div(p.N, BN));
-  int rc;
-  switch (BN) {
-    case 256: rc = launch_cfg<256, 4>(tmA, tmW, p, grid, stream); break;
-    case 128: rc = launch_cfg<128, 3>(tmA, tmW, p, grid, stream); break;
-    case 64:  rc = launch_cfg<64, 4>(tmA, tmW, p, grid, stream); break;
-    default:  rc = launch_cfg<32, 4>(tmA, tmW, p, grid, stream); break;
-  }
-  if (rc) return rc;
-  count_launch();
-  B200VC_LAUNCH_CHECK();
-  return kOk;
+  return tc_launch(p, stream, false);
 }
+
+int tapgemm_tc2_launch(const TgParams& p, cudaStream_t stream) { return tc_launch(p, stream, true); }
+
+void tapgemm_tc2_set_rows256(int on) { g_rows256 = on ? 1 : 0; }
 
 }  // namespace b200vc

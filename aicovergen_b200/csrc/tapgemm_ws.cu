@@ -1,163 +1,36 @@
-// tcgen05 tap-GEMM v3: WEIGHT-STATIONARY + INPUT-HALO kernel for small-channel convolutions (Cout <= 64).
+// wgmma tap-GEMM v3: WEIGHT-STATIONARY + INPUT-HALO kernel for small-channel convolutions (Cout <= 64).
 //
-// The one-tile-per-CTA kernel re-reads the input tile once per tap and the whole weight slab once per tile from L2
-// (profiles/r01: it runs at the L2->SM bandwidth limit, e.g. 432 KB of TMA traffic per 128-pixel tile for the MDX
-// c=48 3x3 layers).  Here:
+// The one-tile-per-CTA kernel re-reads the input tile once per tap and the whole weight slab once per tile from L2.  Here:
 //   * every CTA is persistent and first parks ALL weights of the layer in shared memory (ntaps x kchunks tiles of
-//     [Nr x 32] fp32, <= ~112 KB) — they are never fetched again;
-//   * per output tile (1 x 128 pixel strip) and 32-channel chunk ONE TMA box brings the strip WITH ITS HALO
-//     ([KH rows] x [128 + (KW-1)*dil] pixels x 32 ch); the taps are just row offsets of the UMMA A descriptor inside
-//     that box (the 128-byte swizzle is a function of absolute shared-memory address bits, so shifting the start
-//     address by whole 128-byte rows keeps TMA's layout and the descriptor's view consistent);
-//   * TMEM accumulators are double buffered so the epilogue of tile i overlaps the MMAs of tile i+1; SIXTEEN epilogue
-//     warps (4 per SM sub-partition: lane quarter x 16-column group) keep the register-resident epilogue off the
-//     critical path (ncu r01: with 4 warps the kernel was latency-bound on the epilogue's own instruction stream),
-//     with the bias held in registers across tiles and tile coordinates advanced incrementally (no divisions).
-// L2->SM traffic per tile drops to the halo box only (100 KB instead of 432 KB for MDX c=48; 37 KB instead of 336 KB for
-// the vocoder's C=64 k=7 layers).
-#include "tapgemm.cuh"
-#include <cuda.h>
+//     [Nr x 128 B]) — they are never fetched again;
+//   * per output tile (1 x 128 pixel strip) and 128-byte K chunk ONE TMA box brings the strip WITH ITS HALO
+//     ([KH rows] x [128 + (KW-1)*dil] pixels); the taps are just row offsets of the wgmma A descriptor inside that box
+//     (the 128-byte swizzle is a function of absolute shared-memory address bits, so shifting the start address by whole
+//     128-byte rows keeps TMA's layout and the descriptor's view consistent);
+//   * warpgroup 0 is the TMA producer, warpgroups 1-2 each own 64 rows of the strip and accumulate all taps of a chunk
+//     with m64 x Nr wgmma; the producer keeps fetching the next strips' halo boxes while they run the epilogue.
+// L2->SM traffic per tile drops to the halo box only (for MDX-Net's c=48 3x3 layers ~100 KB instead of ~430 KB).
+#include "hopper.cuh"
 
 namespace b200vc {
 
-int encode_map_f32(CUtensorMap* tm, const void* base, int rank, const cuuint64_t* dims,
-                   const cuuint64_t* strides_bytes, const cuuint32_t* box);   // tapgemm_tc.cu
-int encode_map_f16(CUtensorMap* tm, const void* base, int rank, const cuuint64_t* dims,
-                   const cuuint64_t* strides_bytes, const cuuint32_t* box);   // tapgemm_tc.cu
+using namespace hop;
 
 namespace {
 
-constexpr int KCHUNK = 32;
-constexpr int EPI_WARPS = 16;                      // (TMEM lane quarter) x (16-column group)
-constexpr int NUM_THREADS = 64 + EPI_WARPS * 32;   // warp0 TMA, warp1 MMA, warps 2..17 epilogue
+constexpr int NUM_THREADS = 3 * WG_THREADS;
+constexpr int SMEM_LIMIT = 227 * 1024;
+constexpr int MAX_STAGES = 4;
 
 struct WsGeom {
   int KH, KW, dil_w, dil_h, pad_w, pad_h;
   int BWh;            // halo box width in pixels = 128 + (KW-1)*dil_w
   int a_stage_bytes;  // KH * BWh * 128 rounded up to 1024
   int b_tile_bytes;   // Nr * 128
-  int Nr;             // MMA N (N rounded up to 16)
+  int Nr;             // wgmma N: N rounded up to 16, at least 32
   int stages;
   int total_tiles;
 };
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "LAB_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE;\n\t"
-      "bra LAB_WAIT;\n\t"
-      "DONE:\n\t"
-      "}" ::"r"(bar), "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2,
-                                            int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// fp16 operands (kind::f16): same shared-memory geometry, twice the K per 32-byte step
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32_async(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
 // Tile walker: tile = first + i * stride decomposed into (strip, row, batch) and advanced with carries.
 struct TileWalk {
@@ -177,190 +50,126 @@ struct TileWalk {
   }
 };
 
-// KW_T: the tap-grid width when it is one of the common kernel sizes (3 / 5 / 7 / 11), else 0 = run-time loop.  With
-// Cout <= 64 an MMA lasts 16-32 clk, so the single issuing lane is on the critical path and the tap loop must unroll.
-template <int KW_T, bool F16>
+template <int NR, bool F16>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tapgemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                   const __grid_constant__ TgParams p, const WsGeom g) {
-  constexpr int TM_COLS_PER_ACC = 64;
-  constexpr uint32_t TMEM_COLS = 2 * TM_COLS_PER_ACC;
-
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   constexpr int KE = F16 ? 2 * KCHUNK : KCHUNK;       // K elements per 128-byte chunk row
   constexpr int ES = F16 ? 2 : 4;
   const int kchunks = (p.Kc + KE - 1) / KE;
   const int w_bytes = p.ntaps * kchunks * g.b_tile_bytes;
   const uint32_t w_base = smem_base;                              // resident weights
   const uint32_t a_base = smem_base + w_bytes;                    // A halo ring (w_bytes is a multiple of 1024)
-  const uint32_t bar_base = a_base + g.stages * g.a_stage_bytes;
+  const uint32_t stg_off = w_bytes + g.stages * g.a_stage_bytes;  // two epilogue staging blocks
+  const uint32_t bar_base = smem_base + stg_off + 2 * STG_BYTES;
   auto a_stage = [&](int s) { return a_base + s * g.a_stage_bytes; };
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (4 + s); };
-  const uint32_t w_bar = bar_base + 8u * 8;
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (9 + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (11 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * 13;
+  auto empty_bar = [&](int s) { return bar_base + 8u * (MAX_STAGES + s); };
+  const uint32_t w_bar = bar_base + 8u * 2 * MAX_STAGES;
 
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
+  const int wg = threadIdx.x / WG_THREADS;
   const int ntw = (p.OW + 127) / 128;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
+  if (threadIdx.x == 0) {
+    prefetch_tensormap(&tmA);
+    prefetch_tensormap(&tmW);
     for (int s = 0; s < g.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);              // one arrival per consumer warp
     }
     mbar_init(w_bar, 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 4 * ((p.N + 15) / 16));   // one arrival per participating epilogue warp
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    {
-      // park the whole weight slab: [tap][kchunk] tiles of Nr x 32
-      if (elect_one()) {
-        mbar_expect_tx(w_bar, (uint32_t)w_bytes);
-        for (int j = 0; j < p.ntaps; ++j)
-          for (int kc = 0; kc < kchunks; ++kc)
-            tma_load_3d(w_base + (uint32_t)((j * kchunks + kc) * g.b_tile_bytes), &tmW, w_bar, kc * KE, 0, j);
-      }
-      __syncwarp();
-      int it = 0;
-      const uint32_t a_tx = (uint32_t)(g.KH * g.BWh * 128);
-      TileWalk tk;
-      for (tk.init(blockIdx.x, gridDim.x, g.total_tiles, ntw, p.OH); tk.left > 0; tk.next(ntw, p.OH)) {
-        for (int kc = 0; kc < kchunks; ++kc, ++it) {
-          const int s = it % g.stages;
-          const uint32_t ph = (it / g.stages) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1u);
-          if (elect_one()) {
-            mbar_expect_tx(full_bar(s), a_tx);
-            tma_load_5d(a_stage(s), &tmA, full_bar(s), kc * KE, tk.tw * 128 - g.pad_w, tk.h - g.pad_h, tk.b, 0);
-          }
-          __syncwarp();
-        }
+    setmaxnreg_dec<40>();
+    if (threadIdx.x != 0) return;
+    // park the whole weight slab: [tap][kchunk] tiles of Nr x 128 B
+    mbar_expect_tx(w_bar, (uint32_t)w_bytes);
+    for (int j = 0; j < p.ntaps; ++j)
+      for (int kc = 0; kc < kchunks; ++kc)
+        tma_load_3d(w_base + (uint32_t)((j * kchunks + kc) * g.b_tile_bytes), &tmW, w_bar, kc * KE, 0, j);
+    const uint32_t a_tx = (uint32_t)(g.KH * g.BWh * 128);
+    int s = 0;
+    uint32_t ph = 0;
+    TileWalk tk;
+    for (tk.init(blockIdx.x, gridDim.x, g.total_tiles, ntw, p.OH); tk.left > 0; tk.next(ntw, p.OH)) {
+      for (int kc = 0; kc < kchunks; ++kc) {
+        mbar_wait(empty_bar(s), ph ^ 1u);
+        mbar_expect_tx(full_bar(s), a_tx);
+        tma_load_5d(a_stage(s), &tmA, full_bar(s), kc * KE, tk.tw * 128 - g.pad_w, tk.h - g.pad_h, tk.b, 0);
+        if (++s == g.stages) { s = 0; ph ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // The whole warp walks the loops (warp-uniform control flow keeps descriptors in uniform registers); one elected
-    // lane issues the tcgen05 instructions.
-    {
-      const uint32_t IDESC = F16 ? make_idesc_f16(128, g.Nr) : make_idesc_tf32(128, g.Nr);
-      mbar_wait(w_bar, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      int it = 0, ti = 0;
-      const int my_tiles = (int)blockIdx.x < g.total_tiles ? (g.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-      for (; ti < my_tiles; ++ti) {
-        const int acc = ti & 1;
-        const uint32_t use = (uint32_t)(ti >> 1);
-        mbar_wait(tempty_bar(acc), (use & 1u) ^ 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * TM_COLS_PER_ACC);
-        for (int kc = 0; kc < kchunks; ++kc, ++it) {
-          const int s = it % g.stages;
-          const uint32_t ph = (it / g.stages) & 1;
-          mbar_wait(full_bar(s), ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          // descriptors differ only in their 14-bit start-address field: walk it with adds (this loop runs on one thread)
-          uint64_t adesc_row = make_smem_desc(a_stage(s));
-          uint64_t bdesc = make_smem_desc(w_base + (uint32_t)(kc * g.b_tile_bytes));
-          const uint64_t b_step = (uint64_t)((kchunks * g.b_tile_bytes) >> 4);
-          const uint64_t a_kw_step = (uint64_t)(g.dil_w * 8), a_kh_step = (uint64_t)(g.BWh * 8);   // rows x 128 B >> 4
-          uint32_t accum = kc > 0 ? 1u : 0u;
-          // short last k-chunk (Kc = 48 -> 32 + 16): only the K=8 steps that hold data (25 % fewer MMAs and operand reads)
-          const int nk = (kc == kchunks - 1) ? (((p.Kc - kc * KE) * ES + 31) >> 5) : KCHUNK / 8;
-          if (elect_one()) {
-            for (int kh = 0; kh < g.KH; ++kh, adesc_row += a_kh_step) {
-              uint64_t adesc = adesc_row;
+    return;
+  }
+
+  // ===================== consumers (warpgroups 1, 2) =====================
+  setmaxnreg_inc<232>();
+  const int gi = wg - 1;
+  const int t = threadIdx.x & (WG_THREADS - 1);
+  float* stg = reinterpret_cast<float*>(smem_gen + stg_off + gi * STG_BYTES);
+  // descriptors differ only in their 14-bit start-address field: walk it with adds
+  const uint64_t b_step = (uint64_t)((kchunks * g.b_tile_bytes) >> 4);
+  const uint64_t a_kw_step = (uint64_t)(g.dil_w * 8), a_kh_step = (uint64_t)(g.BWh * 8);   // rows x 128 B >> 4
+  float acc[NR / 2];
 #pragma unroll
-              for (int kw = 0; kw < (KW_T ? KW_T : g.KW); ++kw, adesc += a_kw_step, bdesc += b_step) {
-                if (nk == KCHUNK / 8) {       // full chunk: straight-line issue (a counted loop here costs the N<=32 layers 20 %)
+  for (int i = 0; i < NR / 2; ++i) acc[i] = 0.f;
+  mbar_wait(w_bar, 0);
+  int s = 0;
+  uint32_t ph = 0;
+  TileWalk tk;
+  for (tk.init(blockIdx.x, gridDim.x, g.total_tiles, ntw, p.OH); tk.left > 0; tk.next(ntw, p.OH)) {
+    int prev = -1;
+    for (int kc = 0; kc < kchunks; ++kc) {
+      mbar_wait(full_bar(s), ph);
+      // short last k-chunk (Kc = 48 -> 32 + 16): only the 32-byte K steps that hold data
+      const int nk = (kc == kchunks - 1) ? (((p.Kc - kc * KE) * ES + 31) >> 5) : 4;
+      uint64_t adesc_row = make_desc(a_stage(s) + gi * WG_ROWS * 128);
+      uint64_t bdesc = make_desc(w_base + (uint32_t)(kc * g.b_tile_bytes));
+      uint32_t accum = kc > 0 ? 1u : 0u;
+      fence_operands(acc);
+      wgmma_fence();
+      for (int kh = 0; kh < g.KH; ++kh, adesc_row += a_kh_step) {
+        uint64_t adesc = adesc_row;
+        for (int kw = 0; kw < g.KW; ++kw, adesc += a_kw_step, bdesc += b_step) {
+          if (nk == 4) {
 #pragma unroll
-                  for (int k = 0; k < KCHUNK / 8; ++k) {
-                    if constexpr (F16) umma_f16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), IDESC, accum);
-                    else umma_tf32(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), IDESC, accum);
-                    accum = 1u;
-                  }
-                } else {
-                  for (int k = 0; k < nk; ++k) {
-                    if constexpr (F16) umma_f16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), IDESC, accum);
-                    else umma_tf32(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), IDESC, accum);
-                    accum = 1u;
-                  }
-                }
-              }
+            for (int k = 0; k < 4; ++k) {
+              wgmma<F16, NR>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accum);
+              accum = 1u;
             }
-            umma_commit(empty_bar(s));
-            if (kc == kchunks - 1) umma_commit(tfull_bar(acc));
+          } else {
+            for (int k = 0; k < nk; ++k) {
+              wgmma<F16, NR>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accum);
+              accum = 1u;
+            }
           }
-          __syncwarp();
         }
       }
-    }
-  } else {
-    // ===================== epilogue (warps 2..17) =====================
-    const int q = warp & 3;                         // TMEM lane quarter this warp may read
-    const int n = ((warp - 2) >> 2) * 16;           // its 16-column group
-    if (n < p.N) {
-      float bias16[16];
-      const bool pre_bias = p.bias && !p.bias_per_row && n + 15 < p.N;
-#pragma unroll
-      for (int j = 0; j < 16; ++j) bias16[j] = pre_bias ? __ldg(p.bias + n + j) : 0.f;
-      int ti = 0;
-      TileWalk tk;
-      for (tk.init(blockIdx.x, gridDim.x, g.total_tiles, ntw, p.OH); tk.left > 0; tk.next(ntw, p.OH), ++ti) {
-        const TgRow r = tg_row(p, tk.b, tk.h, tk.tw * 128 + q * 32 + lane);
-        const int acc = ti & 1;
-        const uint32_t use = (uint32_t)(ti >> 1);
-        mbar_wait(tfull_bar(acc), use & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * TM_COLS_PER_ACC + n), v);
-        // registers hold the data: hand the accumulator back to the MMA warp before touching global memory
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        if (lane == 0) mbar_arrive(tempty_bar(acc));
-        tg_store16(p, r, n, v, pre_bias ? bias16 : nullptr, p.N > 32);
+      wgmma_commit();
+      wgmma_wait<1>();                          // the previous chunk's wgmma have retired: its stage can be refilled
+      fence_operands(acc);
+      if (prev >= 0) {
+        __syncwarp();
+        if ((t & 31) == 0) mbar_arrive(empty_bar(prev));
       }
+      prev = s;
+      if (++s == g.stages) { s = 0; ph ^= 1u; }
     }
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+    wgmma_wait<0>();
+    fence_operands(acc);
+    __syncwarp();
+    if ((t & 31) == 0) mbar_arrive(empty_bar(prev));
+    const TgRow r = tg_row(p, tk.b, tk.h, tk.tw * 128 + gi * WG_ROWS + (t & (WG_ROWS - 1)));
+    wg_epilogue<NR>(p, r, 0, acc, stg, 1 + gi);
   }
 }
-
-int num_sms_ws() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
-  }
-  return n;
-}
-
-constexpr int SMEM_LIMIT = 227 * 1024;
 
 // Does the descriptor describe a dense stride-1 convolution over a regular tap grid, small enough for the weights to
 // stay in shared memory?  Fills the geometry when it does.
@@ -385,21 +194,44 @@ bool ws_geometry(const TgParams& p, WsGeom& g) {
   g.pad_w = -p.taps[0].dw; g.pad_h = -p.taps[0].dh;
   g.BWh = 128 + (KW - 1) * dil_w;
   if (g.BWh > 256 || KH > 256) return false;
-  g.Nr = (p.N + 15) & ~15;                 // MMA N and weight-tile rows (16 rows x 128 B = 2 KB granules: stays 1024-aligned)
+  g.Nr = (p.N + 15) & ~15;                 // wgmma N and weight-tile rows (16 rows x 128 B = 2 KB granules: stays 1024-aligned)
+  if (g.Nr < 32) g.Nr = 32;
   g.b_tile_bytes = g.Nr * 128;
   g.a_stage_bytes = ((KH * g.BWh * 128 + 1023) / 1024) * 1024;   // 1024-aligned stages (swizzle atom = 8 rows x 128 B)
   const int ke = (p.dtype & TG_DT_AB) ? 2 * KCHUNK : KCHUNK;
   const int kchunks = (p.Kc + ke - 1) / ke;
   const int w_bytes = p.ntaps * kchunks * g.b_tile_bytes;
-  const int fixed = 8 * 14 + 16 + 1024;
+  const int fixed = 2 * STG_BYTES + 8 * (2 * MAX_STAGES + 1) + 1024;
   int stages = (SMEM_LIMIT - fixed - w_bytes) / g.a_stage_bytes;
-  if (stages > 4) stages = 4;
+  if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages < 2) return false;
   g.stages = stages;
   const long long tiles = (long long)((p.OW + 127) / 128) * p.OH * p.OB;
   if (tiles <= 0 || tiles >= (1ll << 31)) return false;
   g.total_tiles = (int)tiles;
   return true;
+}
+
+template <int NR, bool F16>
+int ws_launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmW, const TgParams& p, const WsGeom& g, int grid, int smem,
+                  cudaStream_t stream) {
+  static bool configured = false;
+  if (!configured) {
+    B200VC_CHECK_CUDA(cudaFuncSetAttribute(tapgemm_ws_kernel<NR, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    configured = true;
+  }
+  tapgemm_ws_kernel<NR, F16><<<grid, NUM_THREADS, smem, stream>>>(tmA, tmW, p, g);
+  return kOk;
+}
+
+template <bool F16>
+int ws_dispatch_nr(const CUtensorMap& tmA, const CUtensorMap& tmW, const TgParams& p, const WsGeom& g, int grid, int smem,
+                   cudaStream_t stream) {
+  switch (g.Nr) {
+    case 32: return ws_launch_cfg<32, F16>(tmA, tmW, p, g, grid, smem, stream);
+    case 48: return ws_launch_cfg<48, F16>(tmA, tmW, p, g, grid, smem, stream);
+    default: return ws_launch_cfg<64, F16>(tmA, tmW, p, g, grid, smem, stream);
+  }
 }
 
 }  // namespace
@@ -409,68 +241,22 @@ bool tapgemm_ws_applicable(const TgParams& p) {
   return ws_geometry(p, g);
 }
 
-template <int KW_T, bool F16>
-static int ws_launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmW, const TgParams& p, const WsGeom& g, int grid, int smem,
-                         cudaStream_t stream) {
-  static bool configured = false;
-  if (!configured) {
-    B200VC_CHECK_CUDA(cudaFuncSetAttribute(tapgemm_ws_kernel<KW_T, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
-    configured = true;
-  }
-  tapgemm_ws_kernel<KW_T, F16><<<grid, NUM_THREADS, smem, stream>>>(tmA, tmW, p, g);
-  return kOk;
-}
-
-template <bool F16>
-static int ws_dispatch_kw(const CUtensorMap& tmA, const CUtensorMap& tmW, const TgParams& p, const WsGeom& g, int grid, int smem,
-                          cudaStream_t stream) {
-  switch (g.KW) {
-    case 3:  return ws_launch_cfg<3, F16>(tmA, tmW, p, g, grid, smem, stream);
-    case 5:  return ws_launch_cfg<5, F16>(tmA, tmW, p, g, grid, smem, stream);
-    case 7:  return ws_launch_cfg<7, F16>(tmA, tmW, p, g, grid, smem, stream);
-    case 11: return ws_launch_cfg<11, F16>(tmA, tmW, p, g, grid, smem, stream);
-    default: return ws_launch_cfg<0, F16>(tmA, tmW, p, g, grid, smem, stream);
-  }
-}
-
 int tapgemm_ws_launch(const TgParams& p, cudaStream_t stream) {
   WsGeom g;
   B200VC_REQUIRE(ws_geometry(p, g), "tapgemm_ws: descriptor is not a small-channel regular convolution");
   const bool f16 = (p.dtype & TG_DT_AB) != 0;
-  const unsigned long long es = f16 ? 2ull : 4ull;
-  const int epb = f16 ? 8 : 4;
   const int ke = f16 ? 2 * KCHUNK : KCHUNK;
   const int kchunks = (p.Kc + ke - 1) / ke;
   CUtensorMap tmA, tmW;
-  {
-    cuuint64_t dims[5], strides[4];
-    cuuint32_t box[5] = {(cuuint32_t)ke, (cuuint32_t)g.BWh, (cuuint32_t)g.KH, 1, 1};
-    long long span = 1;
-    for (int i = 0; i < 5; ++i) {
-      dims[i] = (cuuint64_t)(p.a_dim[i] > 0 ? p.a_dim[i] : 1);
-      if (i > 0) {
-        long long st = p.a_stride[i];
-        if (p.a_dim[i] <= 1) st = ((span + epb - 1) / epb) * epb;
-        strides[i - 1] = (cuuint64_t)st * es;
-        span = st * (long long)dims[i];
-      } else {
-        span = (long long)dims[0];
-      }
-    }
-    int rc = f16 ? encode_map_f16(&tmA, p.A, 5, dims, strides, box) : encode_map_f32(&tmA, p.A, 5, dims, strides, box);
-    if (rc) return rc;
-  }
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)p.Kc, (cuuint64_t)p.N, (cuuint64_t)p.ntaps};
-    cuuint64_t strides[2] = {(cuuint64_t)p.ldw * es, (cuuint64_t)p.wstride * es};
-    cuuint32_t box[3] = {(cuuint32_t)ke, (cuuint32_t)g.Nr, 1};
-    int rc = f16 ? encode_map_f16(&tmW, p.Wt, 3, dims, strides, box) : encode_map_f32(&tmW, p.Wt, 3, dims, strides, box);
-    if (rc) return rc;
-  }
+  const cuuint32_t abox[5] = {(cuuint32_t)ke, (cuuint32_t)g.BWh, (cuuint32_t)g.KH, 1, 1};
+  int rc = encode_a_map(&tmA, p, abox);
+  if (rc) return rc;
+  rc = encode_w_map(&tmW, p, p.ntaps, p.wstride, ke, g.Nr);
+  if (rc) return rc;
   const int w_bytes = p.ntaps * kchunks * g.b_tile_bytes;
-  const int smem = w_bytes + g.stages * g.a_stage_bytes + 8 * 14 + 16 + 1024;
-  const int grid = g.total_tiles < num_sms_ws() ? g.total_tiles : num_sms_ws();
-  int rc = f16 ? ws_dispatch_kw<true>(tmA, tmW, p, g, grid, smem, stream) : ws_dispatch_kw<false>(tmA, tmW, p, g, grid, smem, stream);
+  const int smem = w_bytes + g.stages * g.a_stage_bytes + 2 * STG_BYTES + 8 * (2 * MAX_STAGES + 1) + 1024;
+  const int grid = g.total_tiles < num_sms() ? g.total_tiles : num_sms();
+  rc = f16 ? ws_dispatch_nr<true>(tmA, tmW, p, g, grid, smem, stream) : ws_dispatch_nr<false>(tmA, tmW, p, g, grid, smem, stream);
   if (rc) return rc;
   count_launch();
   B200VC_LAUNCH_CHECK();

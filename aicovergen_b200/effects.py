@@ -2,7 +2,7 @@
 HighpassFilter -> Compressor(ratio 4, threshold -15 dB) -> Reverb; main.py:206-226) and `main.combine_audio` (pydub: gain,
 overlay, export; main.py:229-233) stand.  Kernels: csrc/effects.cu (how each recursion is made parallel is written there).
 
-pedalboard 0.7.7 / JUCE and pydub 0.25.1 are third-party dependencies that are not under /root/reference; what they compute is
+pedalboard 0.7.7 / JUCE and pydub 0.25.1 are third-party dependencies that are not in the reference repository; what they compute is
 restated in oracle/effects.c and oracle/mixdown.py (the latter runs CPython's own `audioop`, so the mix arithmetic is pinned).
 The constants below are computed in float32 the way the JUCE classes compute them."""
 from __future__ import annotations

@@ -1,10 +1,10 @@
-"""B200-native HuBERT-base content encoder — drop-in for the fairseq `HubertModel` object at the plug point
+"""GPU-native HuBERT-base content encoder — drop-in for the fairseq `HubertModel` object at the plug point
 `model.extract_features(source=..., padding_mask=..., output_layer=...)` / `model.final_proj`
 (vc_infer_pipeline.py:398-406; loaded by rvc.load_hubert, rvc.py:98-109).
 
 7-layer strided conv front-end (tap-GEMMs over [T/s, s*C] views), GroupNorm-over-time, grouped
 positional conv (16 groups x 128 taps), 12 post-LN transformer layers with materialised attention
-(QK^T and PV as batched tap-GEMMs, row softmax), all through libb200vc.so on tcgen05 TF32.
+(QK^T and PV as batched tap-GEMMs, row softmax), all through libb200vc.so on wgmma TF32.
 """
 from __future__ import annotations
 

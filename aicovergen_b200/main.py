@@ -218,7 +218,7 @@ def _mdx_model_path(name):
 
 def preprocess_song(song_input, mdx_model_params, song_id, is_webui, input_type, progress=None):
     if input_type == "yt":
-        raise_exception("YouTube download is out of scope for the B200 build (no network stack); pass a local file.", is_webui)
+        raise_exception("YouTube download is out of scope for this build (no network stack); pass a local file.", is_webui)
     orig_song_path, keep_orig = song_input, True
     song_output_dir = os.path.join(output_dir, song_id)
     orig_song_path = convert_to_stereo(orig_song_path)
@@ -287,11 +287,11 @@ def song_cover_pipeline(song_input, voice_model, pitch_change, keep_files, is_we
             raise_exception("Ensure that the song input field and voice model field is filled.", is_webui)
         # options this build does not implement are refused BEFORE any separation / conversion work is done
         if str(song_input).startswith("https://") or str(song_input).startswith("http://"):
-            raise_exception("YouTube input is out of scope for the B200 build; pass a local file.", is_webui)
+            raise_exception("YouTube input is out of scope for this build; pass a local file.", is_webui)
         if pitch_change_all != 0:
-            raise_exception("pitch_change_all needs sox (out of scope for the B200 build).", is_webui)
+            raise_exception("pitch_change_all needs sox (out of scope for this build).", is_webui)
         if f0_method not in SUPPORTED_F0_METHODS:
-            raise_exception(f"f0_method {f0_method!r}: the B200 build runs {SUPPORTED_F0_METHODS}.", is_webui)
+            raise_exception(f"f0_method {f0_method!r}: this build runs {SUPPORTED_F0_METHODS}.", is_webui)
         display_progress("[~] Starting AI Cover Generation Pipeline...", 0, is_webui, progress)
         with open(os.path.join(mdxnet_models_dir, "model_data.json")) as infile:
             mdx_model_params = json.load(infile)

@@ -1,11 +1,11 @@
-"""B200-native MDX-Net separation pass — host mirror of the reference's src/mdx.py (`MDXModel`, `MDX`,
+"""GPU-native MDX-Net separation pass — host mirror of the reference's src/mdx.py (`MDXModel`, `MDX`,
 `run_mdx`, same signatures) over libb200vc.so.
 
 What changes versus the reference is where the work happens: the reference loops chunk by chunk with four
 PCIe crossings per chunk (STFT on GPU -> numpy -> onnxruntime -> torch -> iSTFT -> numpy, mdx.py:187-197).
 Here the song is uploaded once, chunks are gathered in batches straight from HBM (pad_wave zeros + STFT
 reflect padding fused), the STFT / iSTFT are windowed-DFT tap-GEMMs restricted to the dim_f kept bins, the
-TFC-TDF U-Net runs as NHWC tap-GEMMs on tcgen05 with BatchNorm folded, and the iSTFT tail scatters the
+TFC-TDF U-Net runs as NHWC tap-GEMMs on the tensor cores with BatchNorm folded, and the iSTFT tail scatters the
 trimmed chunk directly into the song-level output (trim / concat / [:-pad] / margin logic of mdx.py:195-197,
 107-117 folded into its addressing).  One D2H at the end.
 
@@ -113,7 +113,7 @@ def _stft_gemm(padded, fwd, spec2, model: MDXModel, backend):
     return tg.TapGemm(a, tg.weights(fwd), [(0, 0, 0, 0, 0)], (T, 2, B), o, None, backend, name="mdx.stft")
 
 
-# fp16 storage of the U-Net's activations and GEMM weights (tcgen05 kind::f16, fp32 accumulate): the same 10-bit mantissa
+# fp16 storage of the U-Net's activations and GEMM weights (wgmma f16, fp32 accumulate): the same 10-bit mantissa
 # as the TF32 path at half the shared-memory / L2 / HBM bytes per FLOP.  Only tensors that live inside the network's launch
 # plan change type; the spectrograms on either side stay fp32.
 MDX_FP16 = os.environ.get("B200VC_MDX_FP16", "1") == "1"      # default ON (validated r02: 5.5e-4 rel. on the full-size net, F0 / stems
@@ -128,7 +128,7 @@ class ConvTDFNetB200:
         self.backend = backend
         meta = [int(v) for v in sd["_meta"]]
         (self.dim_f, self.dim_t, self.g, self.l, self.n, self.bn, self.k, self.dim_c) = meta
-        # fp16 storage needs every GEMM of the plan on the TMA/tcgen05 kernels (there is no fp16 SIMT path); the narrowest
+        # fp16 storage needs every GEMM of the plan on the TMA/wgmma kernels (there is no fp16 SIMT path); the narrowest
         # one is the bottleneck TDF with K = dim_f / 2^n / bn (an fp32-operand fallback GEMM when that is not a multiple of 8,
         # which itself needs K % 4 == 0).  Real UVR geometries (dim_f >= 2048) satisfy it; toy geometries fall back to fp32.
         tdf_k = [(self.dim_f >> lvl) // self.bn for lvl in range(self.n + 1)]

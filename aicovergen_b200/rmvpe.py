@@ -1,11 +1,11 @@
-"""B200-native RMVPE F0 estimator — drop-in for the reference `RMVPE` object at the plug point
+"""GPU-native RMVPE F0 estimator — drop-in for the reference `RMVPE` object at the plug point
 `vc.model_rmvpe.infer_from_audio(x, thred=0.03)` (vc_infer_pipeline.py:322-329; rmvpe.py:328-409).
 
 log-mel front-end as a windowed-DFT GEMM, the DeepUnet as NHWC tap-GEMM convolutions with
 BatchNorm folded into the weights, the BiGRU as a cluster kernel, and the cents decode in the
 reference's numpy summation order — all through libb200vc.so.  The decoded F0 feeds an argmax /
 coarse-pitch quantiser whose indices must match the reference bit for bit (BASELINE.json
-north_star), so the U-Net runs on tcgen05 with 3xTF32 split operands (fp32-level accuracy, ~2^-22
+north_star), so the U-Net runs on the tensor cores with 3xTF32 split operands (fp32-level accuracy, ~2^-22
 relative) rather than plain TF32; the front-end DFT, the GRU projections and the salience head
 stay on the exact-fp32 kernel, which is also available for the whole net (backend=BACKEND_SIMT).
 """
@@ -94,7 +94,7 @@ class RMVPEB200:
     def __init__(self, model, is_half: bool = False, device: str = "cuda:0", backend: int = tg.BACKEND_TC,
                  n_blocks: int = 4, n_enc: int = 5, n_inter: int = 4):
         """`model`: path to rmvpe.pt or an already-loaded state dict (E2E(4,1,(2,2)) names).
-        backend = BACKEND_TC (default): the U-Net's convolutions run on tcgen05 as 3xTF32 split-operand GEMMs (fp32-level
+        backend = BACKEND_TC (default): the U-Net's convolutions run on the tensor cores as 3xTF32 split-operand GEMMs (fp32-level
         accuracy, see split3_weights); BACKEND_SIMT: everything on the exact-fp32 FMA kernel (cross-check)."""
         sd = torch.load(model, map_location="cpu") if isinstance(model, (str, bytes)) or hasattr(model, "__fspath__") else model
         self.device = torch.device(device)

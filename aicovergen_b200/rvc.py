@@ -1,5 +1,5 @@
 """Host mirror of the reference's src/rvc.py: `Config`, `load_hubert`, `get_vc`, `rvc_infer` with the same
-signatures and return values, building B200 operator objects instead of torch modules.
+signatures and return values, building GPU operator objects instead of torch modules.
 
   Config(device, is_half)            rvc.py:20-95   -> same attributes; segmentation constants are outputs-defining
   load_hubert(device, is_half, path) rvc.py:98-109  -> HubertB200 (fairseq checkpoint dict {"model": state_dict} or a bare state dict)
@@ -34,7 +34,7 @@ class Config:
     def device_config(self) -> tuple:
         if not torch.cuda.is_available():
             # the reference silently falls back to CPU here (rvc.py:68-71); this build has no CPU path
-            raise RuntimeError("b200vc: no CUDA device available (the B200 hot path has no CPU fallback)")
+            raise RuntimeError("b200vc: no CUDA device available (the GPU hot path has no CPU fallback)")
         i_device = int(str(self.device).split(":")[-1]) if ":" in str(self.device) else 0
         name = torch.cuda.get_device_name(i_device)
         # rvc.py:33-50 forces fp32 on 16xx/10xx/P40 boards (and rewrites training configs, not reproduced)
@@ -56,7 +56,7 @@ class Config:
 
 def load_hubert(device, is_half, model_path):
     """fairseq `checkpoint_utils.load_model_ensemble_and_task([path])` replacement: the checkpoint's "model"
-    state dict is all the B200 encoder needs."""
+    state dict is all the GPU encoder needs."""
     ck = model_path if isinstance(model_path, dict) else torch.load(model_path, map_location="cpu", weights_only=False)
     sd = ck["model"] if isinstance(ck, dict) and "model" in ck else ck
     hubert = HubertB200(sd, device)

@@ -1,9 +1,9 @@
-"""B200-native RVC synthesizer (`net_g`): TextEncoder -> reverse flow -> NSF-HiFiGAN.
+"""GPU-native RVC synthesizer (`net_g`): TextEncoder -> reverse flow -> NSF-HiFiGAN.
 
 Drop-in for the reference's SynthesizerTrnMs{256,768}NSFsid at the operator plug point
 `net_g.infer(feats, p_len, pitch, pitchf, sid)` (vc_infer_pipeline.py:454-465;
 infer_pack/models.py:634-640, 745-751).  Everything numerical runs in libb200vc.so:
-tap-GEMMs on tcgen05 (TF32) plus the fp32 row kernels of ops.py.  This file only
+tap-GEMMs on wgmma (TF32) plus the fp32 row kernels of ops.py.  This file only
 prepares weights (weight-norm folding, packing, flow Flip folding) and sequences launches.
 
 The random draws of the reference (`randn_like` at models.py:748 and :368) are explicit
@@ -41,7 +41,7 @@ def round_tf32(t: torch.Tensor) -> torch.Tensor:
 
 
 # opt-in (round 2): fp16 storage of the vocoder's GEMM-only tensors (the leaky-ReLU copies and the ResBlock mid tensor) and of
-# the ResBlock weights — tcgen05 kind::f16, fp32 accumulate, the residual streams stay fp32.  Validated at the GEMM level only.
+# the ResBlock weights — wgmma f16, fp32 accumulate, the residual streams stay fp32.  Validated at the GEMM level only.
 SYNTH_FP16 = __import__("os").environ.get("B200VC_SYNTH_FP16", "1") == "1"      # default ON from r02e (2.1e-4 abs RMS, same as TF32)
 
 

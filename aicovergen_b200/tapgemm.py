@@ -2,7 +2,7 @@
 
 Everything on the hot path that is a convolution, a linear layer or a batched
 matmul is described by one `b200vc_tapgemm_params` (include/b200vc.h) and run by
-`b200vc_tapgemm` on either the tcgen05 TF32 kernel or the exact-fp32 SIMT
+`b200vc_tapgemm` on either the wgmma TF32 / fp16 kernels or the exact-fp32 SIMT
 kernel.  This module only builds descriptors (pure index arithmetic, testable on
 CPU against torch.nn.functional with tests/emu.py); it never computes.
 

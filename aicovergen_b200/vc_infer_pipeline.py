@@ -1,4 +1,4 @@
-"""Host mirror of the reference's RVC inference driver (src/vc_infer_pipeline.py) over the B200 operators.
+"""Host mirror of the reference's RVC inference driver (src/vc_infer_pipeline.py) over the GPU operators.
 
 Same class, method names, argument order and return types as the reference (`VC(tgt_sr, config)`,
 `VC.pipeline(model, net_g, sid, audio, input_audio_path, times, f0_up_key, f0_method, file_index,
@@ -112,7 +112,7 @@ class VC(object):
             f0 = self.get_f0_crepe_computation(x, f0_min, f0_max, p_len, crepe_hop_length)
         else:
             raise NotImplementedError(
-                f"f0_method={f0_method!r}: 'rmvpe' and 'mangio-crepe' run on the B200 path (pm / harvest / dio / pyin are CPU "
+                f"f0_method={f0_method!r}: 'rmvpe' and 'mangio-crepe' run on the GPU path (pm / harvest / dio / pyin are CPU "
                 "libraries outside the hot path; crepe-tiny and the hybrid methods are not built)")
         return self._coarse_from_f0(f0, f0_up_key, inp_f0)
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native AICoverGen hot path.
+"""bench.py — headline benchmark of the GPU-native (H100) AICoverGen hot path.
 
 Metric (BASELINE.json): audio-seconds/sec (RTF) of the full cover pipeline on a 4-minute 44.1 kHz stereo song.
 One "step" = one 4-min song through the song_cover_pipeline stage graph on one GPU:
@@ -12,6 +12,7 @@ N GPUs = N songs (one per rank, weak scaling, no data-path collective).
   python bench.py --gpus 1 --steps 3 --warmup 3              # our arm
   python bench.py --impl reference --steps 1 --warmup 0      # CPU arm: the oracle restatement of the reference
   python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
+  python bench.py --gpus 1 --steps 3 --warmup 3 --dump-outputs DIR   # + what the last timed step computed, as DIR/*.npy
 Prints ONE JSON line on rank 0.
 """
 from __future__ import annotations
@@ -34,7 +35,7 @@ sys.path.insert(0, ROOT)
 SONG_SECONDS = 240
 SR = 44100
 METRIC = "audio_seconds_per_second_full_cover_pipeline_4min_44k1_stereo"
-DTYPE_NOTE = ("fp16 operands (MDX-Net U-Net, tcgen05 kind::f16) + tf32 (other tensor-core GEMMs; rmvpe as 3xTF32 split operands), fp32 "
+DTYPE_NOTE = ("fp16 operands (MDX-Net U-Net, wgmma f16) + tf32 (other tensor-core GEMMs; rmvpe as 3xTF32 split operands), fp32 "
               "accumulate; fp32/fp64 row kernels")
 UNIT = "audio-s/s"
 
@@ -186,7 +187,7 @@ def output_check(eng, song_dev, song_seconds):
 
 
 def install_tc_profiler():
-    """Wrap TapGemm.__call__ so every tcgen05 launch inside the timed region is bracketed by CUDA events on the
+    """Wrap TapGemm.__call__ so every tensor-core launch inside the timed region is bracketed by CUDA events on the
     launching stream; returns the record list [(kernel family, flops, bytes, start, end)]."""
     from aicovergen_b200 import tapgemm as tg
 
@@ -199,7 +200,7 @@ def install_tc_profiler():
             p = self.params
             if not hasattr(self, "_family"):
                 tile_n = 256 if p.N > 128 else (128 if p.N > 64 else (64 if p.N > 32 else 32))
-                # one family = one kernel template instance: tile width x operand type (kind::f16 and kind::tf32 are different
+                # one family = one kernel template instance: tile width x operand type (f16 and tf32 wgmma are different
                 # kernels with different rooflines)
                 self._family = ("ws" if self.ws_applicable() else f"tc2<{tile_n}>") + ("/f16" if p.dtype & 1 else "/tf32")
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -280,7 +281,8 @@ def peaks():
             d = json.load(f)
         return d, "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA H100 SXM data sheet (700 W): HBM3 bandwidth and dense BF16/FP16 tensor rate; not measured here
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 # --------------------------------------------------------------------------------------------------------------
@@ -378,7 +380,7 @@ def run_reference(args, rank):
                                "CPU time extrapolated from a bounded sample", "sample": vals[-1][2]},
         "cpu_baseline": {"value": v, "unit": UNIT, "cores": threads, "kind": "port",
                          "sample": "EXTRAPOLATED: 1 full-size chunk per MDX model (STFT+net+iSTFT) x chunk count x2 sweeps, + VC.pipeline "
-                                   "(rmvpe, IVF2237 x 87243 index) + effects + mix on 20 s x12; oracle/ restatement pinned against /root/reference",
+                                   "(rmvpe, IVF2237 x 87243 index) + effects + mix on 20 s x12; oracle/ restatement pinned against the reference",
                          "extrapolated": True},
         "e2e": {"value": v, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
@@ -534,6 +536,21 @@ def run_config(args, device):
     print(json.dumps(line), flush=True)
 
 
+DUMP_LIMIT_ELEMS = 12 * 1024 * 1024          # float32 elements per dumped array: 48 MB, under the 64 MB budget
+
+
+def dump_outputs(out_dir: str, cover: torch.Tensor):
+    """cover.npy: the cover's int16 frames [n, 2] as float32 when they fit the budget (a 4-min song does not); otherwise
+    the values at a fixed seeded sorted sample of DUMP_LIMIT_ELEMS flat positions, with cover_shape.npy = [n, 2]."""
+    os.makedirs(out_dir, exist_ok=True)
+    x = cover.detach().float().cpu().numpy()
+    if x.size > DUMP_LIMIT_ELEMS:
+        idx = np.sort(np.random.default_rng(0).choice(x.size, size=DUMP_LIMIT_ELEMS, replace=False))
+        np.save(os.path.join(out_dir, "cover_shape.npy"), np.array(x.shape, dtype=np.float64))
+        x = x.reshape(-1)[idx]
+    np.save(os.path.join(out_dir, "cover.npy"), x.astype(np.float32))
+
+
 # --------------------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -549,6 +566,8 @@ def main():
                     help="weak (default, BASELINE cfg 5): one song per GPU; strong (cfg 4 style): ONE song shared by all GPUs — MDX chunk "
                          "ranges per rank + all-gather, RVC segments round-robin after a broadcast F0")
     ap.add_argument("--no-output-check", action="store_true", help="skip the finite / non-silent / F0-parity check of the timed graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (the cover's int16 frames, as float32) to DIR/*.npy")
     args = ap.parse_args()
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -575,12 +594,14 @@ def main():
             dist.destroy_process_group()
         return
     warm = max(args.warmup, 3)
+    # the synthesizer's noise draws come from torch's generator: seeded, the same arguments give the same outputs every run
+    torch.manual_seed(rank)
     records = install_tc_profiler()
     eng = build_engine(device, rank)
     song = synth_song(args.seconds, seed=rank)
     song_pinned = torch.from_numpy(song).pin_memory()
     song_dev = song_pinned.to(device)
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=device)        # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=device)        # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -617,8 +638,15 @@ def main():
     sampler = ClockSampler(local_rank)
     sampler.start()
     l0 = _ffi.launch_count()
-    dev_ms = timed_loop(lambda: eng.cover_device(song_dev), args.steps)
+    last = {}
+
+    def dev_step():
+        last["cover"] = eng.cover_device(song_dev)
+
+    dev_ms = timed_loop(dev_step, args.steps)
     launches = _ffi.launch_count() - l0
+    if args.dump_outputs and rank == 0 and "cover" in last:
+        dump_outputs(args.dump_outputs, last["cover"])
     # ---- timed: end to end through the public array API with HOST buffers (H2D of the song + D2H of the cover inside)
     out_host = {}
     cover_pinned = torch.empty((song.shape[1] + SR, 2), dtype=torch.int16).pin_memory()      # the caller's result buffer
@@ -628,7 +656,7 @@ def main():
 
     e2e_ms = timed_loop(e2e_step, args.steps)
     sampler.stop()
-    # ---- one more step OUTSIDE the timed regions with CUDA events around every tcgen05 tap-GEMM launch (the event
+    # ---- one more step OUTSIDE the timed regions with CUDA events around every tensor-core tap-GEMM launch (the event
     # pairs perturb launch overlap, so they must not sit inside the step timing): per-kernel-family roofline data
     from aicovergen_b200 import plans
     install_tc_profiler.enabled = True
@@ -655,10 +683,10 @@ def main():
     value = audio_s * args.steps / (dev_ms / 1000.0)
     e2e_value = audio_s * args.steps / (e2e_ms / 1000.0)
 
-    # ---- roofline of the dominant kernel family (tcgen05 tap-GEMM, by tile width) and of the whole step
+    # ---- roofline of the dominant kernel family (tensor-core tap-GEMM, by tile width) and of the whole step
     pk, pk_src = peaks()
     f16_peak = pk["bf16_tflops_sustained"]            # fp16/bf16 dense, measured (sustained figure: kernels timed inside a long step)
-    tf32_peak = f16_peak / 2.0                         # TF32 runs at half the fp16 rate on tcgen05 (nominal ratio; not measured separately)
+    tf32_peak = f16_peak / 2.0                         # TF32 runs at half the fp16 rate on the tensor cores (nominal ratio; not measured separately)
     fam, layer = {}, {}
     for tile_n, fl, by, s, e, is_f16, lname in records:
         ms_i = s.elapsed_time(e)
@@ -674,13 +702,6 @@ def main():
         ly[1] += fl
         ly[2] += 1
     roof, step_roof = None, None
-    traffic = None
-    try:    # per-launch DRAM bytes (dram__bytes_read.sum + dram__bytes_write.sum, one ncu --set full capture) of the
-            # representative launch of the dominant family: profiles/r02_dominant_traffic.json
-        with open(os.path.join(ROOT, "profiles", "r02_dominant_traffic.json")) as f:
-            traffic = json.load(f)
-    except Exception:
-        pass
     if fam:
         top = max(fam.items(), key=lambda kv: kv[1][0])
         tn, (ms, fl, by, cnt, roof_t) = top
@@ -696,30 +717,28 @@ def main():
                   "top_layers_ms": {k: {"ms": round(v[0], 2), "tflops": round(v[1] / v[0] / 1e9, 1), "launches": v[2]} for k, v in top_layers},
                   "profiled_step_ms": round(prof_ms, 1),
                   "flops_note": "2*M*N*K per tap-GEMM launch; the MDX STFT/iSTFT DFT-GEMMs are counted at FFT cost (2.5 n log2 n per frame)"}
-        if traffic and traffic.get("family") == tn:
-            common["traffic_detail"] = traffic
         if tn.startswith("ws") and fl / max(by, 1.0) < 100.0:
             # small-channel convolutions whose arithmetic intensity is below the machine balance -> HBM roofline
             achieved = by / (ms / 1000.0) / 1e9
-            roof = {"kernel": f"tapgemm_ws_kernel [{tn}] (weight-stationary + halo, tcgen05.mma)", "bound": "hbm",
+            roof = {"kernel": f"tapgemm_ws_kernel [{tn}] (weight-stationary + halo, wgmma)", "bound": "hbm",
                     "achieved": round(achieved, 1), "peak": round(pk["hbm_gbs"], 1), "unit": "GB/s",
-                    "frac": round(achieved / pk["hbm_gbs"], 4), "traffic": (traffic or {}).get("dram_bytes_per_launch") if (traffic or {}).get("family") == tn else None,
+                    "frac": round(achieved / pk["hbm_gbs"], 4), "traffic": None,
                     "peak_source": f"{pk_src} hbm_gbs", **common}
         else:
             achieved = fl / (ms / 1000.0) / 1e12
             eff_peak = fl / roof_t if roof_t > 0 else tf32_peak        # FLOP-weighted mix of the fp16 and TF32 peaks (TFLOP/s)
-            roof = {"kernel": (f"tapgemm_ws_kernel [{tn}] (weight-stationary + halo, tcgen05.mma)" if tn.startswith("ws") else
-                               f"tapgemm_tc2_kernel [{tn}] (persistent tcgen05.mma, double-buffered TMEM)"), "bound": "tensor",
+            roof = {"kernel": (f"tapgemm_ws_kernel [{tn}] (weight-stationary + halo, wgmma)" if tn.startswith("ws") else
+                               f"tapgemm_wg_kernel [{tn}] (persistent wgmma)"), "bound": "tensor",
                     "achieved": round(achieved, 2), "peak": round(eff_peak, 1), "unit": "TFLOP/s",
                     "frac": round(achieved / eff_peak, 4),
-                    "traffic": (traffic or {}).get("dram_bytes_per_launch") if (traffic or {}).get("family") == tn else None,
-                    "peak_source": f"{pk_src} bf16_tflops_sustained for kind::f16 kernels, half of it for kind::tf32 kernels "
+                    "traffic": None,
+                    "peak_source": f"{pk_src} bf16_tflops_sustained for f16 kernels, half of it for tf32 kernels "
                                    "(nominal 2:1; a TF32 peak is not in MEASURED_PEAKS.json)", **common}
         step_roof = {"tensor_tflop_per_step": round(tot_fl / 1e12, 2), "gemm_ms_per_step": round(tot_ms, 1),
                      "step_tflops": round(tot_fl / (prof_ms / 1000.0) / 1e12, 1),
                      "frac_of_tensor_roofline_whole_step": round((tot_roof * 1e-12 * 1000.0) / prof_ms, 4),
                      "frac_of_tensor_roofline_inside_gemms": round((tot_roof * 1e-12 * 1000.0) / tot_ms, 4),
-                     "ms_outside_tcgen05_gemms": round(prof_ms - tot_ms, 1)}
+                     "ms_outside_tensor_core_gemms": round(prof_ms - tot_ms, 1)}
 
     if rank == 0:
         line = {
@@ -730,7 +749,7 @@ def main():
                                    "(3072x256/7680, 2048x256/5120, 3072x512/6144; denoise=True) + VC.pipeline (HuBERT-base, rmvpe, "
                                    "IVF2237 x 87243 index_rate 0.5, v2 40k synthesizer) + vocal effects (high-pass, compressor, reverb) "
                                    "+ pydub mix -> int16 cover frames",
-                       "songs": world, "l2": "256 MB buffer written between steps; per-step working set >> 126 MB L2",
+                       "songs": world, "l2": "256 MB buffer written between steps; per-step working set >> 50 MB L2",
                        "weights": "seeded synthetic checkpoints of the real architectures, trained-like (BatchNorm statistics fitted on a calibration clip; smooth single-peak rmvpe salience)"},
             "clocks": sampler.summary(),
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(song.nbytes) * world,

@@ -1,4 +1,4 @@
-/* b200vc — C ABI of the B200-native RVC / MDX hot path.
+/* b200vc — C ABI of the GPU-native (H100, sm_90a) RVC / MDX hot path.
  *
  * The reference (SociallyIneptWeeb/AICoverGen) is pure Python; its "operator
  * boundary" for this path is the set of library calls it makes into
@@ -42,11 +42,11 @@ enum {
 /* which kernel family executes a tap-GEMM */
 enum {
   B200VC_BACKEND_SIMT_FP32 = 0, /* exact fp32 FMA kernel                      */
-  B200VC_BACKEND_TC_TF32 = 1,   /* tcgen05.mma kind::tf32, TMA-fed, TMEM accumulators. Picks the weight-stationary +
-                                   halo kernel (tapgemm_ws.cu) for small-channel regular convolutions, else the
-                                   one-tile-per-CTA kernel (tapgemm_tc.cu)                                          */
-  B200VC_BACKEND_TC_TF32_PERSISTENT = 2, /* persistent double-buffered-TMEM variant (tapgemm_tc2.cu), development     */
-  B200VC_BACKEND_TC_TF32_TILE = 3,       /* force tapgemm_tc.cu                                                       */
+  B200VC_BACKEND_TC_TF32 = 1,   /* wgmma (TF32, or fp16 per `dtype`), TMA-fed, fp32 register accumulators. Picks the
+                                   weight-stationary + halo kernel (tapgemm_ws.cu) for small-channel regular
+                                   convolutions, else the persistent kernel (tapgemm_tc.cu)                         */
+  B200VC_BACKEND_TC_TF32_PERSISTENT = 2, /* persistent launch of tapgemm_tc.cu (one CTA per SM walks the tiles)        */
+  B200VC_BACKEND_TC_TF32_TILE = 3,       /* one tile per CTA launch of tapgemm_tc.cu                                  */
   B200VC_BACKEND_TC_TF32_WS = 4          /* force tapgemm_ws.cu (error if the descriptor does not qualify)            */
 };
 
@@ -106,11 +106,10 @@ typedef struct b200vc_tapgemm_params {
                            loads; 2 = out/res2 (and a layout-sharing out2) channels-last + 16-byte aligned; 4 = per-column
                            bias float4-loadable; 8 = own-layout out2 channels-last + aligned; 16 = res likewise        */
   int32_t round_tf32;   /* bit0: round `out` to TF32 (RN), bit1: round `out2` — for tensors only consumed by TF32 GEMMs */
-  int32_t dtype;        /* element types (0 = everything fp32): bit0 A and W are IEEE fp16 (tcgen05 kind::f16, fp32
+  int32_t dtype;        /* element types (0 = everything fp32): bit0 A and W are IEEE fp16 (wgmma f16, fp32
                            accumulate; same 10-bit mantissa as TF32 at half the operand bytes) — tensor-core backends
                            only; bit1 out, bit2 out2, bit3 res, bit4 res2 are fp16.  Pointers stay typed `float*` in
-                           this struct; offsets and strides are in ELEMENTS of the tensor's own type.
-                           EXPERIMENTAL in round 1: compiled and emulator-tested, not yet validated on a GPU. */
+                           this struct; offsets and strides are in ELEMENTS of the tensor's own type. */
   int32_t split;        /* 3xTF32 split-operand storage (fp32 accuracy on the TF32 tensor core: x = hi + lo with hi = RN_tf32(x),
                            lo = RN_tf32(x - hi); a consumer GEMM reads the K-concatenation [hi | lo | hi] against weights
                            [W_hi | W_hi | W_lo], i.e. hi.W_hi + lo.W_hi + hi.W_lo, dropping only lo.W_lo ~ 2^-22):
@@ -152,9 +151,9 @@ int b200vc_plan_destroy(b200vc_plan* plan);
 
 /* ---- tap-GEMM ---- */
 int b200vc_tapgemm(const b200vc_tapgemm_params* p, int backend, void* stream);
-/* experimental: let the persistent tcgen05 kernel use 256-row tiles (two MMAs per weight tile); off by default */
+/* experimental: let the persistent tensor-core kernel use 256-row tiles (one weight tile feeds two 128-row blocks); off by default */
 int b200vc_tapgemm_set_rows256(int on);
-/* 1 when the descriptor satisfies the TMA alignment rules of the tcgen05 path */
+/* 1 when the descriptor satisfies the TMA alignment rules of the tensor-core path */
 int b200vc_tapgemm_tc_supported(const b200vc_tapgemm_params* p);
 /* 1 when the descriptor is a small-channel regular convolution the weight-stationary kernel handles */
 int b200vc_tapgemm_ws_applicable(const b200vc_tapgemm_params* p);

@@ -2,8 +2,8 @@
 (`VC.get_f0_crepe_computation`, vc_infer_pipeline.py:96-137, selected at :310-313).
 
 The reference's own lines (quantile normalisation, the `torchcrepe.predict` call with `batch_size = hop_length * 2`,
-`pad=True`, the `source < 0.001 -> nan` rule and the `np.interp` resize) are restated from /root/reference.  Everything
-inside `torchcrepe.predict` is a THIRD-PARTY dependency absent from /root/reference — `torchcrepe==0.0.20`
+`pad=True`, the `source < 0.001 -> nan` rule and the `np.interp` resize) are restated from the reference repository.  Everything
+inside `torchcrepe.predict` is a THIRD-PARTY dependency absent from the reference repository — `torchcrepe==0.0.20`
 (requirements.txt:19) — restated here from its published source (torchcrepe/{core,model,decode,convert}.py and
 librosa.sequence.viterbi): PARITY UNPINNED (no torchcrepe, no librosa, no `full.pth` in this environment):
 

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — small DSP restatements of third-party helpers the reference calls.
 
-librosa 0.9.1 (requirements.txt) is not installed and not under /root/reference: these follow
+librosa 0.9.1 (requirements.txt) is not installed and not in the reference repository: these follow
 its published algorithms; PARITY UNPINNED against the real librosa.
 """
 from __future__ import annotations
@@ -78,7 +78,7 @@ def pcm16_soundfile(x: np.ndarray) -> np.ndarray:
     """`soundfile.write(path, float_array, sr)` to a .wav (default subtype PCM_16; mdx.py:273,280): python-soundfile enables
     libsndfile's clipping for every file it opens (`sf_command(SFC_SET_CLIPPING, SF_TRUE)`), so floats are converted by
     pcm.c f2s_clip_array: scaled = x * (8.0 * 0x10000000) in float; >= 0x7FFFFFFF -> 0x7FFF; <= -8.0 * 0x10000000 -> 0x8000;
-    else lrintf(scaled) >> 16.  soundfile / libsndfile are absent from /root/reference and from this image: restated from
+    else lrintf(scaled) >> 16.  soundfile / libsndfile are absent from the reference repository: restated from
     their published sources, PARITY UNPINNED."""
     s = np.asarray(x, dtype=np.float32) * np.float32(8.0 * 0x10000000)
     out = np.empty(s.shape, dtype=np.int16)

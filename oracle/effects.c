@@ -6,7 +6,7 @@
  *     with AudioFile(in) as f, AudioFile(out, 'w', f.samplerate, f.num_channels) as o:
  *         while f.tell() < f.frames: o.write(board(f.read(int(f.samplerate)), f.samplerate, reset=False))
  *
- * `pedalboard==0.7.7` (requirements.txt:11) is a third-party dependency, absent from /root/reference and from this image; it
+ * `pedalboard==0.7.7` (requirements.txt:11) is a third-party dependency, absent from the reference repository; it
  * wraps JUCE 6 DSP classes.  Their published algorithms are restated below — PARITY UNPINNED (restated from the published
  * sources of pedalboard / JUCE; nothing here was executed against them):
  *

@@ -2,7 +2,7 @@
 (hubert_base: conv feature extractor mode "default", post-LN transformer) as called at
 vc_infer_pipeline.py:398-406.
 
-fairseq is a third-party dependency absent from /root/reference (requirements.txt:2) -> restated from the
+fairseq is a third-party dependency absent from the reference repository (requirements.txt:2) -> restated from the
 published architecture; cross-checked against transformers.HubertModel (tests/test_oracle_vs_reference.py);
 PARITY UNPINNED against real fairseq.  State-dict names are fairseq's (SURVEY.md B9).
 """

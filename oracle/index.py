@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — numpy restatement of the faiss calls on the RVC path.
 
-faiss-cpu 1.7.3 (requirements.txt:3) is a third-party dependency absent from /root/reference: the
+faiss-cpu 1.7.3 (requirements.txt:3) is a third-party dependency absent from the reference repository: the
 `added_IVF{n}_Flat_nprobe_1_*.index` files (rvc_models/MODELS.txt, README.md:165) are IndexIVFFlat / L2 /
 nprobe=1, restated from the published algorithm; PARITY UNPINNED against real faiss (tie order in
 particular).  Call sites: vc_infer_pipeline.py:505-507 (read_index, reconstruct_n), :421 (search k=8).

@@ -3,7 +3,7 @@
 * `stft` / `istft`, `segment`, `pad_wave`, `process_wave`, the `run_mdx` arithmetic: follow mdx.py:19-54,
   92-235, 257-280 and are pinned against the reference's own classes (tests/test_oracle_vs_reference.py).
 * `convtdfnet`: the TFC-TDF U-Net that lives inside the UVR-MDX-NET `.onnx` files (mdx.py:74-77,
-  download_models.py:23-26).  The ONNX graphs are not in /root/reference and onnxruntime is not installed:
+  download_models.py:23-26).  The ONNX graphs are not in the reference repository and onnxruntime is not installed:
   restated from the public KUIELab / UVR "ConvTDFNet" architecture (SURVEY.md §8(c)); PARITY UNPINNED.
 """
 from __future__ import annotations

@@ -5,7 +5,7 @@
     inst   = AudioSegment.from_wav(instrumental)    - 7 + inst_gain
     main.overlay(backup).overlay(inst).export(path, format=...)
 
-`pydub==0.25.1` (requirements.txt:12) is a third-party dependency that is absent from /root/reference and from this image.
+`pydub==0.25.1` (requirements.txt:12) is a third-party dependency that is absent from the reference repository.
 Its sample arithmetic is CPython's `audioop` C module, which IS in this image (Python 3.12 stdlib) and is called here
 directly, so every sample operation (`mul`, `ratecv`, `tostereo`, `add`) is the reference's own code: PINNED.  The glue around
 it is restated from pydub's published source (audio_segment.py: `apply_gain`, `_sync`, `set_channels`, `set_frame_rate`,

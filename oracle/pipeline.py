@@ -2,8 +2,8 @@
 oracle restatements of its operators (oracle/hubert.py, rmvpe.py, synth.py, index.py).
 
 Pinned against the reference's own `VC.pipeline` run unmodified with duck-typed operators
-(tests/test_oracle_vs_reference.py, tools/make_golden.py).  It is also what bench.py times as the CPU
-baseline / `--impl reference` arm on the GPU box, where /root/reference does not exist.
+(tools/make_golden.py, tests/test_oracle_vs_reference.py).  It is also what bench.py times as the CPU
+baseline / `--impl reference` arm.
 """
 from __future__ import annotations
 

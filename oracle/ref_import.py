@@ -1,8 +1,8 @@
-"""TEST INFRASTRUCTURE ONLY — import the *unmodified* reference modules from /root/reference.
+"""TEST INFRASTRUCTURE ONLY — import the *unmodified* reference modules from a checkout of the reference repository
+named by the environment variable AICOVERGEN_REFERENCE.
 
-Only usable in the build container (the GPU box has no /root/reference).  It is how the
-oracle restatements in this directory are pinned and how tests/golden/*.npz are generated
-(tools/make_golden.py).  Recipe follows SURVEY.md Appendix B10: third-party modules that are
+It is how tests/golden/*.npz, which pin the oracle restatements in this directory, are generated
+(tools/make_golden.py); the tests themselves only read those files.  Recipe follows SURVEY.md Appendix B10: third-party modules that are
 not installed (faiss, librosa, parselmouth, pyworld, torchcrepe, onnxruntime, soundfile,
 fairseq) are replaced by inert stubs; nothing of the reference's own arithmetic is touched.
 """
@@ -16,12 +16,12 @@ import types
 
 import numpy as np
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("AICOVERGEN_REFERENCE", "")
 REF_SRC = os.path.join(REF_ROOT, "src")
 
 
 def available() -> bool:
-    return os.path.isdir(REF_SRC)
+    return bool(REF_ROOT) and os.path.isdir(REF_SRC)
 
 
 def _stub(name: str, **attrs):
@@ -53,7 +53,7 @@ def setup():
     if _done:
         return
     if not available():
-        raise RuntimeError("/root/reference is not present on this machine")
+        raise RuntimeError("set AICOVERGEN_REFERENCE to a checkout of the reference repository")
     if not hasattr(np, "int"):
         np.int = int  # vc_infer_pipeline.py:368 uses the removed alias
     import transformers  # noqa: F401  (must be imported before librosa is stubbed: it probes it via find_spec)

@@ -1,5 +1,5 @@
-"""Helpers to run the UNMODIFIED reference (from /root/reference) with duck-typed operators.
-Only usable where /root/reference exists (build container). TEST INFRASTRUCTURE ONLY."""
+"""Helpers to run the UNMODIFIED reference (oracle/ref_import.py) with duck-typed operators, for tools/make_golden.py.
+Only usable where a reference checkout is available. TEST INFRASTRUCTURE ONLY."""
 import types
 
 import numpy as np

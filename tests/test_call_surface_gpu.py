@@ -112,7 +112,9 @@ def test_file_level_call_surface(tmp_path, monkeypatch):
     # ---------------- rvc.Config / load_hubert / get_vc / rvc_infer --------------------------------------------------
     config = brvc.Config("cuda:0", True)
     assert (config.x_pad, config.x_query, config.x_center, config.x_max) == (3, 10, 60, 65)
-    assert config.n_cpu > 0 and config.gpu_mem > 100 and config.device == "cuda:0"
+    # rvc.py:53-60, 89: whole GiB of the device, rounded as the reference rounds; > 4 GiB selects the (3, 10, 60, 65) segmentation
+    gib = int(torch.cuda.get_device_properties(0).total_memory / 1024 / 1024 / 1024 + 0.4)
+    assert config.n_cpu > 0 and config.gpu_mem == gib and config.gpu_mem > 4 and config.device == "cuda:0"
     hubert = brvc.load_hubert("cuda:0", config.is_half, os.path.join(rvc_dir, "hubert_base.pt"))
     cpt_l, version, net_g, tgt_sr, vc = brvc.get_vc("cuda:0", config.is_half, config, os.path.join(rvc_dir, "Synth", "Synth.pth"))
     assert (version, tgt_sr, cpt_l["config"][-3]) == ("v2", 40000, 109) and isinstance(vc, brvc.VC)

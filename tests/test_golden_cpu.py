@@ -1,5 +1,5 @@
 """The oracle restatements reproduce the golden vectors generated from the UNMODIFIED reference
-(tools/make_golden.py) — runs anywhere, no GPU, no /root/reference."""
+(tools/make_golden.py) — runs anywhere, no GPU, no reference checkout."""
 import os
 
 import numpy as np

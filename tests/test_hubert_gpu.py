@@ -1,4 +1,4 @@
-"""GPU parity: B200 HuBERT (extract_features plug point) vs the CPU oracle restatement (oracle/hubert.py,
+"""GPU parity: HuBERT (extract_features plug point) vs the CPU oracle restatement (oracle/hubert.py,
 cross-checked against transformers.HubertModel).  BASELINE.json config 2: 30 s of 16 kHz audio."""
 import numpy as np
 import pytest

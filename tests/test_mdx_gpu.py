@@ -1,4 +1,4 @@
-"""GPU parity: B200 MDX pass (ConvTDFNet, STFT/iSTFT, chunked process_wave / run_mdx arithmetic) vs the CPU
+"""GPU parity: MDX pass (ConvTDFNet, STFT/iSTFT, chunked process_wave / run_mdx arithmetic) vs the CPU
 oracle (oracle/mdx.py; stft/istft/chunking pinned against src/mdx.py)."""
 import numpy as np
 import pytest
@@ -133,7 +133,7 @@ def test_first_and_final_conv_row_kernels():
 
 @pytest.mark.parametrize("cfg", [dict(dim_f=256, dim_t=32, g=8, n=3), dict(dim_f=3072, dim_t=256, g=48, n=5)])
 def test_convtdfnet_parity_fp16_storage(cfg, monkeypatch):
-    """The U-Net with fp16 activation / weight storage (tcgen05 kind::f16, fp32 accumulate) — the DEFAULT mode — on
+    """The U-Net with fp16 activation / weight storage (wgmma f16, fp32 accumulate) — the DEFAULT mode — on
     trained-like checkpoints: same mantissa width as the TF32 path, half the bytes."""
     import aicovergen_b200.mdx as bm
     from oracle import mdx as om

@@ -1,6 +1,6 @@
 """The MDX U-Net launch plan (aicovergen_b200/mdx.py: _NetPlan) executed on CPU: every tap-GEMM through the descriptor
 emulator, the two pointwise row kernels through torch.  Checks, without a GPU, that the plan computes the oracle's network
-and — for the fp16-storage mode — that every GEMM in it is addressable by the TMA/tcgen05 kernels (the fp16 path has no
+and — for the fp16-storage mode — that every GEMM in it is addressable by the TMA/wgmma kernels (the fp16 path has no
 SIMT fallback)."""
 import pytest
 import torch

@@ -1,82 +1,83 @@
-"""Pins the oracle restatements against the UNMODIFIED reference code imported from /root/reference
-(build container only; skipped on the GPU box)."""
+"""Pins the oracle restatements against what the UNMODIFIED reference code computes on the same seeded inputs.  The
+reference outputs are stored in tests/golden/oracle_pins.npz (tools/make_golden.py pins): bit-exact comparisons as the
+SHA-256 of the reference tensor, tolerance comparisons on a fixed seeded sample of output positions."""
+import hashlib
 import os
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
-pytestmark = pytest.mark.reference
+G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-def test_synth_oracle_matches_reference():
+@pytest.fixture(scope="module")
+def pins():
+    return np.load(os.path.join(G, "oracle_pins.npz"))
+
+
+def _sha(t):
+    a = t.numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def test_synth_oracle_matches_reference(pins):
     from aicovergen_b200.synthetic import make_rvc_checkpoint
     from oracle import synth as osyn
-    from refshim import ref_net_g
 
     cpt = make_rvc_checkpoint("40k", "v2")
-    net = ref_net_g(cpt)
     P = 48
     g = torch.Generator().manual_seed(1)
     phone = torch.randn(1, P, 768, generator=g)
     pitch = torch.randint(1, 255, (1, P), generator=g)
     pitchf = torch.rand(1, P, generator=g) * 300 + 80
     pitchf[:, 7:15] = 0
-    torch.manual_seed(11)
-    with torch.no_grad():
-        o_ref = net.infer(phone, torch.tensor([P]), pitch, pitchf, torch.tensor([0]))[0]
     nz, ns = osyn.draw_noise(11, P, 192, 400)
-    o = osyn.infer(cpt, phone, pitch, pitchf, torch.tensor([0]), nz, ns)
-    assert (o - o_ref).abs().max().item() < 2e-6
+    o = osyn.infer(cpt, phone, pitch, pitchf, torch.tensor([0]), nz, ns).numpy().ravel()
+    assert o.size == int(pins["synth_n"])
+    assert np.abs(o[pins["synth_idx"]] - pins["synth_out"]).max() < 2e-6
 
 
-def test_synthetic_checkpoints_load_strictly_in_reference():
+def test_synthetic_checkpoints_load_strictly_in_reference(pins):
+    """Every parameter the reference modules declare (name and shape) is in the synthetic checkpoints, and nothing else."""
     from aicovergen_b200.synthetic import make_rmvpe_state_dict, make_rvc_checkpoint
-    from oracle import ref_import
+
+    def names(sd):
+        return sorted(f"{k}:{tuple(v.shape)}" for k, v in sd.items())
 
     for key, up in (("40k", 400), ("48k_v2", 480), ("32k", 320)):
         cpt = make_rvc_checkpoint(key, "v2")
-        m = ref_import.module("infer_pack.models")
-        net = m.SynthesizerTrnMs768NSFsid(*cpt["config"], is_half=False)
-        del net.enc_q
-        res = net.load_state_dict(cpt["weight"], strict=False)
-        assert not res.missing_keys and not res.unexpected_keys, (key, res)
+        assert names(cpt["weight"]) == list(pins[f"params_{key}"]), key
         assert int(np.prod(cpt["config"][12])) == up
-    r = ref_import.module("rmvpe")
-    r.E2E(4, 1, (2, 2)).load_state_dict(make_rmvpe_state_dict(), strict=True)
+    assert names(make_rmvpe_state_dict()) == list(pins["params_rmvpe"])
 
 
-def test_rmvpe_oracle_matches_reference():
+def test_rmvpe_oracle_matches_reference(pins):
     from aicovergen_b200.synthetic import make_rmvpe_state_dict
     from oracle import rmvpe as orm
-    from refshim import ref_rmvpe, vocal_like
+    from siggen import vocal_like
 
     sd = make_rmvpe_state_dict()
-    rm = ref_rmvpe(sd)
     x = vocal_like(2.5)
-    f_ref = rm.infer_from_audio(x, 0.03)
+    f_ref = pins["rmvpe_f0"]
     f_or = orm.infer_from_audio(sd, x, 0.03)
     assert f_ref.shape == f_or.shape
     assert np.abs(f_ref - f_or).max() / f_ref.max() < 1e-5
-    with torch.no_grad():
-        mel = rm.mel_extractor(torch.from_numpy(x)[None])
-        assert torch.equal(mel, orm.log_mel(torch.from_numpy(x)[None]))
-        h = rm.mel2hidden(mel)[0].numpy()
+    assert _sha(orm.log_mel(torch.from_numpy(x)[None])) == str(pins["rmvpe_mel_sha"])
     # decode restatement is bit-exact given the same salience
-    assert np.array_equal(rm.decode(h.copy(), 0.03), orm.decode(h.copy(), 0.03))
+    h = pins["rmvpe_salience"]
+    assert np.array_equal(orm.decode(h.copy(), 0.03), pins["rmvpe_decode"])
 
 
 @pytest.mark.parametrize("with_index", [False, True])
-def test_pipeline_oracle_matches_reference(with_index):
+def test_pipeline_oracle_matches_reference(pins, with_index):
     """Whole VC.pipeline: 2 segments (small x_* so it stays cheap), rmvpe F0, protect + RMS mix (+ index)."""
     from aicovergen_b200.synthetic import (make_hubert_state_dict, make_ivf_index_data, make_rmvpe_state_dict,
                                            make_rvc_checkpoint)
     from oracle import hubert as ohub
     from oracle import pipeline as opipe
     from oracle.index import IvfFlatIndex
-    from refshim import HubertShim, ref_net_g, ref_rmvpe, ref_vc, vocal_like
+    from siggen import vocal_like
 
     hsd = make_hubert_state_dict(layers=2)
     cpt = make_rvc_checkpoint("40k", "v2")
@@ -84,77 +85,46 @@ def test_pipeline_oracle_matches_reference(with_index):
     audio = vocal_like(5.3)
     xs = dict(x_pad=1, x_query=1, x_center=2, x_max=3)
     index = None
-    file_index = ""
-    vmod, vc = ref_vc(40000, **xs)
     if with_index:
         base = ohub.extract_features(hsd, torch.from_numpy(vocal_like(3.0, seed=3))[None], 2)[0]
         cent, vecs = make_ivf_index_data(base, n_total=2000, nlist=40)
         index = IvfFlatIndex(cent, vecs)
-        tmp = tempfile.NamedTemporaryFile(suffix=".index", delete=False)
-        tmp.close()
-        file_index = tmp.name
-        sys.modules["faiss"].read_index = lambda p: index
-    vc.model_rmvpe = ref_rmvpe(rsd)
-    # HubertShim with only 2 transformer layers: output_layer=12 would overrun -> wrap
-    class Shim(HubertShim):
-        def extract_features(self, source, padding_mask, output_layer):
-            return (ohub.extract_features(self.sd, source.float(), 2), padding_mask)
-    net_g = ref_net_g(cpt)          # built BEFORE seeding: module construction consumes RNG draws
-    torch.manual_seed(5)
-    out_ref = vc.pipeline(Shim(hsd), net_g, 0, audio.copy(), "x.wav", [0, 0, 0], 0, "rmvpe", file_index,
-                          0.5, 1, 3, 40000, 0, 0.25, "v2", 0.33, 128)
-    # oracle with the same 2-layer hubert: temporarily patch the layer count
+    # the same 2-layer hubert the reference run used: temporarily patch the layer count
     orig = ohub.extract_features
     ohub.extract_features = lambda sd, src, layer=12, n_heads=12: orig(sd, src, 2, n_heads)
     try:
         out, info = opipe.pipeline(hsd, cpt, rsd, audio.copy(), index=index, seed=5, return_all=True, **xs)
     finally:
         ohub.extract_features = orig
-        if with_index:
-            os.unlink(file_index)
+    k = f"pipeline_{int(with_index)}"
     assert len(info["opt_ts"]) >= 1, "test must exercise the cut-point path"
-    assert out.shape == out_ref.shape and out.dtype == np.int16
-    diff = np.abs(out.astype(np.int32) - out_ref.astype(np.int32))
+    assert out.size == int(pins[k + "_n"]) and out.dtype == np.int16
+    diff = np.abs(out[pins[k + "_idx"]].astype(np.int32) - pins[k + "_out"].astype(np.int32))
     # the only arithmetic difference is fp32 reassociation in the GRU restatement (f0 differs ~1e-6 relative,
     # which the random-weight synthesizer amplifies to ~1e-4 on the waveform)
     assert diff.max() <= 12, diff.max()
     assert np.sqrt((diff.astype(np.float64) ** 2).mean()) < 1.5
 
 
-def test_mdx_oracle_matches_reference():
+def test_mdx_oracle_matches_reference(pins):
     """mdx.py's own MDXModel.stft/istft and MDX.process_wave (2 threads, margins, padding) with a fake ORT
     session running the restated net, vs oracle/mdx.py."""
     from aicovergen_b200.synthetic import make_mdx_state_dict
     from oracle import mdx as om
-    from oracle import ref_import
 
-    ref = ref_import.module("mdx")
     dim_f, dim_t, n_fft = 256, 16, 2048         # small geometry: chunk = 1024*15 samples, trim 1024
     sd = make_mdx_state_dict(dim_f=dim_f, dim_t=dim_t, g=8, n=3)
     net = lambda spec: om.convtdfnet(sd, spec)
-
-    class FakeSession:
-        def __init__(self, path, providers=None):
-            pass
-
-        def run(self, _, feed):
-            return [net(torch.from_numpy(feed["input"])).numpy()]
-
-    sys.modules["onnxruntime"].InferenceSession = FakeSession
-    ref.ort.InferenceSession = FakeSession
-    model = ref.MDXModel(torch.device("cpu"), dim_f=dim_f, dim_t=dim_t, n_fft=n_fft, stem_name="Vocals", compensation=1.035)
-    sess = ref.MDX("fake.onnx", model, processor=-1)
     mp = om.MdxParams(dim_f, dim_t, n_fft, stem_name="Vocals", compensation=1.035)
     rng = np.random.default_rng(0)
     N = 44100 * 3 + 1234
     wave = (rng.standard_normal((2, N)) * 0.2).astype(np.float32)
     # stft / istft
     x = torch.from_numpy(wave[:, :mp.chunk_size].copy())[None]
-    assert torch.equal(model.stft(x), mp.stft(x))
     spec = mp.stft(x)
-    assert torch.allclose(model.istft(spec), mp.istft(spec), atol=0, rtol=0)
+    assert _sha(spec) == str(pins["mdx_stft_sha"])
+    assert _sha(mp.istft(spec)) == str(pins["mdx_istft_sha"])
     # full process_wave
-    ref_out = sess.process_wave(wave.copy(), 2)
     got = om.process_wave(wave.copy(), mp, net, 2)
-    assert ref_out.shape == got.shape == wave.shape
-    assert np.abs(ref_out - got).max() < 1e-6
+    assert tuple(pins["mdx_shape"]) == got.shape == wave.shape
+    assert np.abs(got.ravel()[pins["mdx_idx"]] - pins["mdx_out"]).max() < 1e-6

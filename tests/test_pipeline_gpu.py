@@ -1,4 +1,4 @@
-"""GPU parity of the whole RVC path: VC.pipeline (B200 operators) vs oracle/pipeline.py (pinned against the
+"""GPU parity of the whole RVC path: VC.pipeline (GPU operators) vs oracle/pipeline.py (pinned against the
 reference's unmodified VC.pipeline).  Bar (BASELINE.json north_star): coarse F0 indices bit-exact, fp32 waveform
 within 1e-3 RMS."""
 import os

@@ -1,4 +1,4 @@
-"""GPU parity: B200 RMVPE (infer_from_audio plug point) vs the CPU oracle restatement (oracle/rmvpe.py,
+"""GPU parity: RMVPE (infer_from_audio plug point) vs the CPU oracle restatement (oracle/rmvpe.py,
 pinned against src/rmvpe.py).  BASELINE.json config 1: 10 s 100->1000 Hz sine sweep at 16 kHz."""
 import numpy as np
 import pytest
@@ -37,7 +37,7 @@ def test_rmvpe_f0_parity(seconds, weights):
     f0_ref = orm.decode(hid_ref.numpy().copy(), 0.03)
     pitch_ref, pitchf_ref = orm.coarse_pitch(f0_ref, 0)
 
-    # trained-like weights: the default backend (U-Net on tcgen05, 3xTF32 split operands); round-1 raw weights: the exact-fp32
+    # trained-like weights: the default backend (U-Net on the tensor cores, 3xTF32 split operands); round-1 raw weights: the exact-fp32
     # SIMT kernel (their unstructured salience head turns any rounding difference into a different octave)
     net = RMVPEB200(sd, device="cuda:0", backend=tg.BACKEND_TC if weights == "trained_like" else tg.BACKEND_SIMT)
     sal = net.salience_from_audio(torch.from_numpy(x).cuda()).cpu()
@@ -46,13 +46,21 @@ def test_rmvpe_f0_parity(seconds, weights):
     f0 = net.infer_from_audio(x, thred=0.03)
     assert f0.shape == f0_ref.shape == (1 + len(x) // 160,)
     pitch, pitchf = orm.coarse_pitch(f0, 0)
-    mism = int((pitch != pitch_ref).sum())
+    # A frame whose reference F0 lies within 1e-6 relative of a rounding boundary of the quantiser is a tie at float32
+    # resolution (one float32 ulp is ~6e-8 relative; the salience it is decoded from is float32 and carries the tolerance
+    # asserted below): no fp32 implementation can place it reliably, so there either neighbouring index is accepted.
+    # The 10 s sweep has one such frame (74: 4.3e-8 relative from the boundary); every other frame must match exactly.
+    up, dn = orm.coarse_pitch(f0_ref * (1 + 1e-6), 0)[0], orm.coarse_pitch(f0_ref * (1 - 1e-6), 0)[0]
+    tie = up != dn
+    mism = int(((pitch != pitch_ref) & ~tie).sum())
     both = (f0 > 0) & (f0_ref > 0)
     rel = np.abs(f0 - f0_ref)[both] / f0_ref[both]
-    print(f"[rmvpe {weights} {seconds}s] coarse-pitch mismatches {mism}/{len(pitch)}; f0 max rel diff {rel.max():.3e}; voiced "
-          f"{(f0_ref > 0).mean():.2f}; {len(np.unique(pitch_ref))} distinct levels")
+    print(f"[rmvpe {weights} {seconds}s] coarse-pitch mismatches {mism}/{len(pitch)} (+ {int((pitch != pitch_ref)[tie].sum())} of "
+          f"{int(tie.sum())} float32 ties); f0 max rel diff {rel.max():.3e}; voiced {(f0_ref > 0).mean():.2f}; "
+          f"{len(np.unique(pitch_ref))} distinct levels")
     assert err < (1.5e-3 if weights == "trained_like" else 3e-4)
     assert mism == 0, "coarse pitch indices must match the reference bit for bit"
+    assert ((pitch == up) | (pitch == dn))[tie].all(), "a tie frame must take one of the two indices it lies between"
     assert np.array_equal(f0 > 0, f0_ref > 0) and rel.max() < 1e-3
 
 
@@ -77,7 +85,7 @@ def test_rmvpe_net_parity_given_logmel(kind, backend, bar):
     err = (got - ref).abs().max().item()
     f0, f0_ref = net.decode(got.numpy()), orm.decode(ref.numpy().copy(), 0.03)
     mism = int((orm.coarse_pitch(f0)[0] != orm.coarse_pitch(f0_ref)[0]).sum())
-    print(f"[rmvpe net {'3xTF32 tcgen05' if backend == tg.BACKEND_TC else 'fp32 simt'} | oracle log-mel, {kind}] salience max abs err {err:.3e}; "
+    print(f"[rmvpe net {'3xTF32 wgmma' if backend == tg.BACKEND_TC else 'fp32 simt'} | oracle log-mel, {kind}] salience max abs err {err:.3e}; "
           f"coarse-pitch mismatches {mism}/{len(f0)}")
     assert got.shape == ref.shape and err < bar and mism == 0
     # the front-end alone: device log-mel vs torch.stft log-mel on bins above the clamp region

@@ -1,4 +1,4 @@
-"""GPU parity: B200 synthesizer (net_g.infer plug point) vs the CPU oracle restatement
+"""GPU parity: synthesizer (net_g.infer plug point) vs the CPU oracle restatement
 (oracle/synth.py, pinned against infer_pack/models.py) on seeded synthetic weights."""
 import pytest
 import torch

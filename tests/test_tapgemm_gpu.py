@@ -1,4 +1,4 @@
-"""GPU parity of the tap-GEMM kernels (SIMT fp32 and tcgen05 TF32) through the C ABI,
+"""GPU parity of the tap-GEMM kernels (SIMT fp32 and wgmma TF32 / fp16) through the C ABI,
 against torch CPU fp32 convolutions on the same seeded inputs."""
 import pytest
 import torch
@@ -268,8 +268,8 @@ def test_conv_transpose2d_k2s2_two_gemms(bname, backend, tol, B, H, W, Ci, Co):
 @pytest.mark.parametrize("T,Ci,Co,k", [(50000, 64, 160, 3), (41000, 96, 96, 5), (45000, 32, 48, 3), (70001, 32, 32, 1)])
 def test_persistent_256_row_tiles_conv1d(T, Ci, Co, k):
     """(experimental path, enabled through b200vc_tapgemm_set_rows256)
-    Problems with >= #SM 256-row tiles take the two-MMAs-per-B-tile path of the persistent kernel (BN 256: single
-    TMEM stage; BN <= 128: double-buffered); checked against the exact-fp32 SIMT kernel on the same device."""
+    Problems with >= #SM 256-row tiles take the path of the persistent kernel where one B tile feeds two 128-row blocks
+    (BN <= 128; BN 256 keeps 128-row tiles); checked against the exact-fp32 SIMT kernel on the same device."""
     g = torch.Generator().manual_seed(T)
     x, w, b = torch.randn(T, Ci, generator=g), torch.randn(Co, Ci, k, generator=g) / (Ci * k) ** 0.5, torch.randn(Co, generator=g)
     res = torch.randn(T, Co, generator=g)
@@ -308,7 +308,7 @@ def test_persistent_256_row_tiles_conv2d():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# fp16 operand storage (tcgen05 kind::f16): the default storage of the MDX-Net U-Net from round 2 on.
+# fp16 operand storage (wgmma f16): the default storage of the MDX-Net U-Net from round 2 on.
 # ------------------------------------------------------------------------------------------------------------------
 import os  # noqa: E402
 

@@ -223,7 +223,7 @@ def test_conv_transpose2d_k2s2_two_gemms_with_mapped_skip():
 
 def test_fp16_tensors_descriptor_and_semantics():
     """fp16 operands / outputs / residual (b200vc.h `dtype`): flags, element-unit offsets and the same epilogue
-    semantics, executed by the emulator on half tensors (the tcgen05 kind::f16 path itself needs a GPU)."""
+    semantics, executed by the emulator on half tensors (the wgmma f16 path itself needs a GPU)."""
     g = torch.Generator().manual_seed(21)
     B, H, W, Ci, Co = 1, 6, 40, 48, 32
     x = torch.randn(B, H, W, Ci, generator=g).half()

@@ -38,7 +38,7 @@ def main():
     ap.add_argument("--only", default="", help="substring filter on the shape name")
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--warm", type=int, default=3)
-    ap.add_argument("--fp16", action="store_true", help="fp16 operand / activation storage (tcgen05 kind::f16)")
+    ap.add_argument("--fp16", action="store_true", help="fp16 operand / activation storage (wgmma f16)")
     args = ap.parse_args()
     global WARM, ITERS, DT
     DT = torch.float16 if args.fp16 else torch.float32

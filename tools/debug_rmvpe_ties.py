@@ -1,4 +1,4 @@
-"""How often does the coarse pitch of the B200 rmvpe differ from the CPU oracle, and is every difference an fp32
+"""How often does the coarse pitch of the GPU rmvpe differ from the CPU oracle, and is every difference an fp32
 near-tie of the salience argmax?  (random-weight nets have noise-like salience, SURVEY.md §7.3 item 1)"""
 import os
 import sys

@@ -1,5 +1,5 @@
 """fp16-storage safety probe for the MDX U-Net (CPU, test infrastructure): runs the oracle network on one chunk and records
-max |value| of every tensor the B200 plan would STORE in fp16 mode (post-activation conv outputs, the TDF hidden layer after
+max |value| of every tensor the GPU plan would STORE in fp16 mode (post-activation conv outputs, the TDF hidden layer after
 the s2 scaling, block outputs x + tdf(x), the skip product).  fp16 overflows at 65504; values far below that are safe.
 usage: python tools/mdx_activation_range.py [--dim-f 3072 --dim-t 256 --g 48] [--real-stft]"""
 import argparse
